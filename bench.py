@@ -2,6 +2,7 @@
 """bench.py -- forward+backward Gaussians/s of the strand-aligned rasterizer hot path.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl mine|reference] [--mode native|render|render_hair]
+                    [--dump-outputs DIR]
 
 Workload (BASELINE.json configs[2], the one `metric` is quoted on): 500 000 synthetic strand-aligned
 Gaussians (SURVEY.md 8d scene "strands(5000)"), 1920x1080, one ring camera per step, forward +
@@ -13,9 +14,15 @@ tensor copied from pinned host memory and the loss read back every step.
 N > 1 (torchrun, one rank per GPU): views shard one per rank per step (weak scaling), the flat
 gradient arena is summed with ONE NCCL all-reduce per step; time is the max over ranks.
 
-`--impl reference` times Oracle-A: the reference's own CUDA extension compiled in place for sm_100a
+`--impl reference` times Oracle-A: the reference's own CUDA extension compiled in place for sm_90a
 (oracle/_ref) -- the reference ships no CPU rasterizer, so that build is the baseline
 (BASELINE.json north_star).  It prints the same JSON line with "impl": "reference".
+
+The headline figure is ONE window of exactly K timed steps (`--repeats R` times it R times and reports the
+median window).  `--dump-outputs DIR` then writes what the last timed step returned to its caller (the
+rendered image, radii and every gradient of the backward) as DIR/<name>.npy in float32; arrays are
+sampled at fixed, seeded positions so that the dump stays under 64 MB.  Inputs are seeded: two builds run
+with the same arguments can be compared output for output.
 
 Prints ONE JSON line on rank 0.
 """
@@ -27,6 +34,7 @@ import os
 import statistics
 import subprocess
 import sys
+import tempfile
 import time
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
@@ -56,14 +64,16 @@ def parse_args():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-roofline", action="store_true")
     ap.add_argument("--ref-steps", type=int, default=10)
-    ap.add_argument("--repeats", type=int, default=5, help="how many times the timed K-step window is repeated (median reported)")
+    ap.add_argument("--repeats", type=int, default=1, help="how many times the timed K-step window is repeated (median reported)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32, <= 64 MB in all)")
     ap.add_argument("--collective", default="auto", choices=["auto", "peer-mc", "peer-nomc", "nccl"],
                     help="N>1: gh_allreduce_p2p over symmetric memory (auto: peer ld/st up to 4 GPUs, NVLS multimem from 8) or NCCL")
     return ap.parse_args()
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries, sampled every 100 ms)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -71,7 +81,7 @@ class ClockSampler:
     def __init__(self, gpu_index: int):
         self.gpu = gpu_index
         self.proc = None
-        self.path = f"/tmp/gh_clocks_{os.getpid()}.csv"
+        self.path = os.path.join(tempfile.gettempdir(), f"gh_clocks_{os.getpid()}.csv")
 
     def start(self):
         try:
@@ -119,7 +129,29 @@ def measured_peak_gbs():
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3)"
+
+
+DUMP_BUDGET_BYTES = 63 * 1000 * 1000        # all dumped files together stay under 64 MB
+
+
+def dump_outputs(out_dir, arrays):
+    """Write each array as out_dir/<name>.npy (float32).  An array larger than its share of the budget is
+    sampled at sorted positions drawn from a generator seeded by its name and size, so that the same
+    positions are written by every run with the same arguments; <name>_index.npy holds them."""
+    import zlib
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    share = DUMP_BUDGET_BYTES // (12 * len(arrays))       # float32 value + float64 index of a sampled element
+    for name, t in arrays.items():
+        flat = t.detach().reshape(-1).float()
+        if flat.numel() > share:
+            rng = np.random.default_rng(zlib.crc32(f"{name}:{flat.numel()}".encode()))
+            idx = np.sort(rng.choice(flat.numel(), size=share, replace=False))
+            np.save(os.path.join(out_dir, f"{name}_index.npy"), idx.astype(np.float64))
+            flat = flat[torch.from_numpy(idx).to(flat.device)]
+        np.save(os.path.join(out_dir, f"{name}.npy"), flat.cpu().numpy())
 
 
 def algorithmic_bytes(P, R, W, H, T, mode):
@@ -282,6 +314,7 @@ def main():
         else:
             last["grads"] = mod.rasterize_gaussians_backward(*bw)
         last["R"] = R
+        last["out"] = (color, radii)
         return R
 
     def timed(nsteps, fn):
@@ -321,6 +354,17 @@ def main():
             gpu_launches = int(_capi.load().gh_kernel_launch_count() - launches0)
     clocks = sampler.stop() if rank == 0 else None
     ms_total = statistics.median(windows)
+    if args.dump_outputs and rank == 0:
+        # what the last timed step returned: the image, radii and the gradients of the backward
+        color, radii = last["out"]
+        arrays = {"color": color, "radii": radii}
+        if isinstance(last["grads"], tuple):       # the 9-tuple of rasterize_gaussians_backward
+            names = ("means2D", "colors", "opacity", "means3D", "cov3D", "conic", None, "scales", "rotations")
+            arrays.update({n: g for n, g in zip(names, last["grads"]) if n is not None})
+        else:
+            arrays.update(last["views"])
+        dump_outputs(args.dump_outputs, arrays)
+        log(f"[bench] outputs of the last timed step written to {args.dump_outputs}")
     ms_per_step = ms_total / args.steps
     n_eff = N if args.impl == "mine" else 1       # reference arm: rank 0 alone runs (one GPU's worth of work)
     value = (args.steps * P * n_eff) / (ms_total * 1e-3)
@@ -516,15 +560,8 @@ def main():
             gbs = stage_bytes[name] / (avg * 1e-3) / 1e9 if avg > 0 else 0.0
             stages[name] = {"ms": avg, "alg_bytes": int(stage_bytes[name]), "gbs": gbs, "frac": gbs / peak}
         dom = max(stages, key=lambda k: stages[k]["ms"])
-        traffic = None
-        try:     # DRAM bytes per launch of that kernel from the committed ncu --set full capture
-            import glob
-            tf = sorted(glob.glob(os.path.join(ROOT, "profiles", "r*_traffic.json")))[-1]
-            traffic = json.load(open(tf)).get(dom) if args.mode == "native" else None
-        except Exception:
-            traffic = None
         roofline = {"bound": "hbm", "kernel": dom, "achieved": stages[dom]["gbs"], "peak": peak, "unit": "GB/s",
-                    "frac": stages[dom]["frac"], "traffic": traffic, "peak_source": peak_src,
+                    "frac": stages[dom]["frac"], "peak_source": peak_src,
                     "ms": stages[dom]["ms"], "alg_bytes": stages[dom]["alg_bytes"],
                     "timing": f"CUDA events around each stage on the launching stream, {nrf} steps after the timed region"}
     if use_dist:
@@ -543,7 +580,7 @@ def main():
             cpu_baseline = {"value": ref_value, "unit": UNIT, "cores": sm_count, "kind": "reference",
                             "ms_per_step": ms_ref / args.ref_steps,
                             "sample": f"{args.ref_steps} steps of the same workload; the reference has no CPU rasterizer, "
-                                      f"this is its own CUDA extension (oracle/_ref, sm_100a) on the same B200, {sm_count} SMs"}
+                                      f"this is its own CUDA extension (oracle/_ref, sm_90a) on the same GPU, {sm_count} SMs"}
             log(f"[bench] reference CUDA build: {ms_ref / args.ref_steps:.3f} ms/step -> {ref_value / 1e6:.1f} M Gaussians/s")
         else:
             cpu_baseline = {"value": None, "unit": UNIT, "cores": sm_count, "kind": "reference",
@@ -795,7 +832,8 @@ def main():
             "config": {"workload": f"strands({args.strands}) = {P_total} Gaussians, {W}x{H}, fwd+bwd, mode={args.mode}",
                        "gaussians_per_view": P, "num_rendered": int(last["R"]), "views_cycled": args.views,
                        "parallelism": f"views sharded one per GPU (dp{N}), one all-reduce of the gradient arena per step: {collective}" if N > 1 else "single GPU",
-                       "l2": "per-step footprint ~0.3 GB (83 MB image + 83 MB upstream grad + 68 MB grads + inputs/workspaces) > 126 MB L2; views cycled"},
+                       "l2": "per-step footprint ~0.3 GB (83 MB image + 83 MB upstream grad + 68 MB grads + inputs/workspaces) > 50 MB L2; views cycled"},
+            "gpu": torch.cuda.get_device_name(device),
             "clocks": clocks,
             "e2e": e2e,
             "gpu_launches": gpu_launches,

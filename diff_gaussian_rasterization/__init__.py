@@ -2,7 +2,7 @@
 
     from diff_gaussian_rasterization import GaussianRasterizationSettings, GaussianRasterizer
 
-Putting this repository's root on `sys.path` makes that import resolve to the B200-native
+Putting this repository's root on `sys.path` makes that import resolve to the H100-native
 implementation in `gaussianhaircut_b200` -- nothing in the reference's Python needs to change.
 """
 from gaussianhaircut_b200.rasterizer import (  # noqa: F401

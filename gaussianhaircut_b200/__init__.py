@@ -1,4 +1,4 @@
-"""gaussianhaircut_b200 -- B200-native (sm_100a) strand-aligned differentiable Gaussian rasterizer.
+"""gaussianhaircut_b200 -- H100-native (sm_90a) strand-aligned differentiable Gaussian rasterizer.
 
 A from-scratch replacement for the one hot path of eth-ait/GaussianHaircut: the extension
 `ext/diff_gaussian_rasterization_hair` behind `src/gaussian_renderer`.  The public surface mirrors

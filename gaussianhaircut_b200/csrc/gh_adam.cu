@@ -147,7 +147,7 @@ extern "C" int gh_adam_step(int n_groups, float* const* params, const float* con
     unsigned long long largest = 0;
     for (int k = 0; k < n_groups; k++) largest = sizes[k] > largest ? sizes[k] : largest;
     const unsigned long long want = (largest / 4 + 255) / 256;
-    const dim3 grid((unsigned int)(want < 1 ? 1 : (want > 148ull * 8 ? 148ull * 8 : want)), (unsigned int)n_groups);
+    const dim3 grid((unsigned int)(want < 1 ? 1 : (want > 132ull * 8 ? 132ull * 8 : want)), (unsigned int)n_groups);
     if (nan_flag) {
         if (cudaMemsetAsync(nan_flag, 0, sizeof(unsigned int), stream) != cudaSuccess)
             return gh_set_error(GH_E_CUDA, "gh_adam_step: memset of the NaN flag failed");

@@ -234,9 +234,9 @@ extern "C" int gh_allreduce_p2p(const unsigned long long* peer_bufs, const unsig
     }
     float* mc = reinterpret_cast<float*>(multicast_buf);
     // every CTA waits for the entry barrier, so all of them must be resident: sms x (CTAs that fit per SM, capped)
-    // defaults = the fastest point of the measured sweep at 8 GPUs / 42 MB (tools/allreduce_case.py --sweep, profiles/):
-    // the NVLS path is fastest with FEW requests in flight (128 threads, 1 CTA per SM, 2 x 16 B per thread: 121 us against
-    // 148 us at 256 threads x 4 CTAs x 8); the peer load/store path wants one full CTA per SM
+    // defaults (tunable through the environment, swept by tools/allreduce_case.py --sweep; not yet re-swept on H100
+    // machines): the NVLS path with FEW requests in flight (128 threads, 1 CTA per SM, 2 x 16 B per thread); the peer
+    // load/store path with one full CTA per SM
     const int threads = gh_env_int("GH_ALLREDUCE_THREADS", mc ? 128 : 512, 32, GH_AR_MAX_THREADS) & ~31;
     const int mc_u = gh_env_int("GH_ALLREDUCE_UNROLL", 2, 1, 16);
     const int want_cps = gh_env_int("GH_ALLREDUCE_CTAS_PER_SM", 1, 1, 8);

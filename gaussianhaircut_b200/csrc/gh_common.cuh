@@ -1,4 +1,4 @@
-// Shared device/host definitions for the B200-native strand-aligned Gaussian rasterizer.
+// Shared device/host definitions for the H100-native strand-aligned Gaussian rasterizer.
 //
 // Replaces (as a fresh design, not a translation) the per-stage plumbing of the reference's
 // ext/diff_gaussian_rasterization_hair/cuda_rasterizer/{config.h, auxiliary.h, rasterizer_impl.h}.

@@ -15,7 +15,7 @@
 //     gh_loss_presum_kernel    sum of the orientation weights (the gradient needs 1 / sum)
 //     gh_loss_pointwise_kernel masked L1 value, mask L1, orientation loss -> loss sums, dL/dout channels 3..9
 //     gh_loss_main_kernel      SSIM statistics (separable 11-tap window, register
-//                              blocked over shared memory, packed FP32) -> SSIM sum, three derivative maps
+//                              blocked over shared memory, float2 pairs) -> SSIM sum, three derivative maps
 //     gh_loss_ssim_bwd_kernel  second separable pass over the derivative maps -> dL/dout channels 0..2
 //     gh_loss_finalize_kernel  scalars; zeroes the orientation gradients if Lorient was NaN
 // Output channel layout (SRC/gaussian_renderer/__init__.py:98): image 0..2, mask 3..4, dir 5..7,
@@ -44,6 +44,9 @@ enum { GH_LS_W = 0, GH_LS_L1 = 1, GH_LS_SSIM = 2, GH_LS_MASK = 3, GH_LS_ORIENT =
 
 __device__ __forceinline__ float gh_sign(float x) { return (x > 0.f) ? 1.f : ((x < 0.f) ? -1.f : 0.f); }
 __device__ __forceinline__ float2 gh_l2(float a) { return make_float2(a, a); }
+// (x, y) pairs filtered together; each half is one IEEE-rounded FMUL / FFMA
+__device__ __forceinline__ float2 gh_mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 gh_fma2(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
 
 __device__ __forceinline__ void gh_block_add(double v, double* dst, double* s_part) {
     // 256-thread CTA: warp shuffle tree, then one atomic per CTA
@@ -153,7 +156,7 @@ gh_loss_pointwise_kernel(GhLossParams prm, const float* __restrict__ out, const 
 
 // SSIM statistics of a 32x32 tile: separable 11-tap window, register blocked (a thread filters 8
 // adjacent columns of a halo row, then 4 adjacent rows of a column, so a shared-memory value is reused
-// by up to 8 taps) and packed: (x, y) and (x^2, y^2) travel as float2 through FFMA2.
+// by up to 8 taps) and paired: (x, y) and (x^2, y^2) travel as float2.
 template <int MINB>
 __global__ void __launch_bounds__(256, MINB)
 gh_loss_main_kernel(GhLossParams prm, const float* __restrict__ out, const float* __restrict__ gt_image,
@@ -220,14 +223,14 @@ gh_loss_main_kernel(GhLossParams prm, const float* __restrict__ out, const float
 #pragma unroll
             for (int k = 0; k < 18; k++) {
                 const float2 v = sXY[r][8 * gq + k];
-                const float2 sq = __fmul2_rn(v, v);
+                const float2 sq = gh_mul2(v, v);
                 const float xy = v.x * v.y;
 #pragma unroll
                 for (int o = 0; o < 8; o++) {
                     if (k - o >= 0 && k - o <= 10) {
                         const float gk = prm.g[k - o];
-                        s01[o] = __ffma2_rn(gh_l2(gk), v, s01[o]);
-                        s23[o] = __ffma2_rn(gh_l2(gk), sq, s23[o]);
+                        s01[o] = gh_fma2(gh_l2(gk), v, s01[o]);
+                        s23[o] = gh_fma2(gh_l2(gk), sq, s23[o]);
                         s4[o] = fmaf(gk, xy, s4[o]);
                     }
                 }
@@ -250,8 +253,8 @@ gh_loss_main_kernel(GhLossParams prm, const float* __restrict__ out, const float
                 for (int o = 0; o < 4; o++) {
                     if (k - o >= 0 && k - o <= 10) {
                         const float gk = prm.g[k - o];
-                        m4[o] = __ffma2_rn(gh_l2(gk), a01, m4[o]);
-                        e4[o] = __ffma2_rn(gh_l2(gk), a23, e4[o]);
+                        m4[o] = gh_fma2(gh_l2(gk), a01, m4[o]);
+                        e4[o] = gh_fma2(gh_l2(gk), a23, e4[o]);
                         e12_4[o] = fmaf(gk, a4, e12_4[o]);
                     }
                 }
@@ -349,7 +352,7 @@ gh_loss_ssim_bwd_kernel(GhLossParams prm, const float* __restrict__ out, const f
 #pragma unroll
                 for (int o = 0; o < 8; o++) {
                     if (k - o >= 0 && k - o <= 10) {
-                        s01[o] = __ffma2_rn(gh_l2(prm.g[k - o]), v, s01[o]);
+                        s01[o] = gh_fma2(gh_l2(prm.g[k - o]), v, s01[o]);
                         s2[o] = fmaf(prm.g[k - o], u, s2[o]);
                     }
                 }
@@ -371,7 +374,7 @@ gh_loss_ssim_bwd_kernel(GhLossParams prm, const float* __restrict__ out, const f
 #pragma unroll
                 for (int o = 0; o < 4; o++) {
                     if (k - o >= 0 && k - o <= 10) {
-                        D01_4[o] = __ffma2_rn(gh_l2(prm.g[k - o]), a01, D01_4[o]);
+                        D01_4[o] = gh_fma2(gh_l2(prm.g[k - o]), a01, D01_4[o]);
                         D2_4[o] = fmaf(prm.g[k - o], a2, D2_4[o]);
                     }
                 }
@@ -456,12 +459,12 @@ extern "C" int gh_image_loss(int width, int height, const float* out_color, cons
     const size_t plane = (size_t)width * height;
     if (cudaMemsetAsync(sums, 0, GH_LS_COUNT * sizeof(double), stream) != cudaSuccess)
         return gh_set_error(GH_E_CUDA, "gh_image_loss: memset of the partial sums failed");
-    const int rb = (int)((plane + 255) / 256 < 148u * 8u ? (plane + 255) / 256 : 148u * 8u);
+    const int rb = (int)((plane + 255) / 256 < 132u * 8u ? (plane + 255) / 256 : 132u * 8u);
     gh_loss_presum_kernel<<<rb, 256, 0, stream>>>(gt_orient_conf, plane, sums);
     const dim3 grid((width + GH_LT - 1) / GH_LT, (height + GH_LT - 1) / GH_LT), block(256);
-    const int pb = (int)((plane + 255) / 256 < 148u * 16u ? (plane + 255) / 256 : 148u * 16u);
+    const int pb = (int)((plane + 255) / 256 < 132u * 16u ? (plane + 255) / 256 : 132u * 16u);
     gh_loss_pointwise_kernel<<<pb, 256, 0, stream>>>(prm, out_color, gt_image, gt_mask, gt_orient_angle, gt_orient_conf, sums, dL_dout);
-    // 4 CTAs per SM (64 registers): measured 279 us per call at 1080p against 299 (2 CTAs) / 326 (3 CTAs)
+    // 4 CTAs per SM (64 registers)
     gh_loss_main_kernel<4><<<grid, block, 0, stream>>>(prm, out_color, gt_image, gt_mask, sums, dmaps);
     gh_loss_ssim_bwd_kernel<4><<<grid, block, 0, stream>>>(prm, out_color, gt_image, gt_mask, dmaps, dL_dout);
     gh_loss_finalize_kernel<<<rb, 256, 0, stream>>>(prm, sums, losses, dL_dout);

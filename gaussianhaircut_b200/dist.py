@@ -8,7 +8,7 @@ A training step consumes one camera (src/train_gaussians.py:103-110) and cameras
 given the same Gaussians, so the path shards by view with no collective inside the op.  The only
 exchange is the sum of the per-Gaussian gradients, which the backward already writes into one flat
 float32 arena (`_C.rasterize_gaussians_backward_arena`): the arena IS the NCCL buffer, no packing
-copy.  torch.distributed (NCCL over NVLink/NVSwitch on the B200 box, gloo in CPU tests) is plumbing.
+copy.  torch.distributed (NCCL over NVLink/NVSwitch, gloo in CPU tests) is plumbing.
 """
 from __future__ import annotations
 

@@ -1,5 +1,5 @@
 /*
- * gh_rasterizer.h -- C ABI of libgh_raster.so, the B200-native (sm_100a) strand-aligned
+ * gh_rasterizer.h -- C ABI of libgh_raster.so, the H100-native (sm_90a) strand-aligned
  * differentiable Gaussian rasterizer.
  *
  * Drop-in boundary.  These entry points are what the reference's native binding for this path

@@ -16,7 +16,7 @@ with the two shims the container needs (SURVEY.md section 0.7):
     uint32_t without the include).
 
 Flags follow torch's CUDAExtension defaults (no fast-math, -fmad=true, IEEE
-div/sqrt) plus `-gencode arch=compute_100a,code=sm_100a`.
+div/sqrt) plus `-gencode arch=compute_90a,code=sm_90a`.
 
 `oracle/_ref/` is git-ignored (build output) but travels to the GPU box.
 The reference has no CPU implementation of this path, so this CUDA build is
@@ -99,7 +99,8 @@ def build(verbose: bool = True, force: bool = False) -> str:
         os.path.join(REF_EXT, "ext.cpp"),
     ]
     stage_python(verbose=False)
-    deps = srcs + [os.path.join(HERE, "glm_shim", "glm", "glm.hpp")]
+    # this file holds the flags (target architecture): an oracle/_ref built with other flags is rebuilt
+    deps = srcs + [os.path.join(HERE, "glm_shim", "glm", "glm.hpp"), os.path.abspath(__file__)]
     if is_built() and not force:
         newest = max(os.path.getmtime(p) for p in deps)
         if os.path.getmtime(SO_PATH) >= newest:
@@ -116,7 +117,7 @@ def build(verbose: bool = True, force: bool = False) -> str:
     nvcc_flags = ["-D__CUDA_NO_HALF_OPERATORS__", "-D__CUDA_NO_HALF_CONVERSIONS__",
                   "-D__CUDA_NO_BFLOAT16_CONVERSIONS__", "-D__CUDA_NO_HALF2_OPERATORS__",
                   "--expt-relaxed-constexpr", "-std=c++17", "-O3",
-                  "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+                  "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
                   "--compiler-options", "-fPIC", "-include", "cstdint", "-w"]
     cxx_flags = ["-std=c++17", "-O2", "-fPIC", "-include", "cstdint", "-w"]
 

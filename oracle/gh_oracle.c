@@ -9,7 +9,7 @@
  *
  * Pinning.  The reference ships no tests or golden vectors for this path.  This restatement is
  * pinned against (a) tests/golden/ *.npz, outputs of the reference extension itself executed on a
- * B200 (tests/golden/make_golden.py), and (b) the reference authors' own PyTorch restatement of
+ * GPU (tests/golden/make_golden.py), and (b) the reference authors' own PyTorch restatement of
  * stage 1 (src/scene/gaussian_model.py:143-337), see tests/test_oracle_cpu.py.
  *
  * Rounding.  Everything that feeds a decision of the reference (depth key bits, tile rectangle,

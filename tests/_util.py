@@ -115,6 +115,147 @@ def rel_err(a: torch.Tensor, b: torch.Tensor) -> float:
     return d / nb
 
 
+# ------------------------------------------------------------------ compact records of reference outputs
+# The reference outputs the parity tests compare against are stored under tests/golden/ as records small enough
+# to keep in the repository, whatever the size of the array:
+#   digest  sha256 of the raw bytes (bit-exact comparisons),
+#   norm    L2 norm, absmax, shape,
+#   proj    SKETCH_K projections on pseudo-random +-1 vectors: the mean square of <r, a> - <r, ref> over the K
+#           vectors estimates ||a - ref||^2 (Johnson-Lindenstrauss), i.e. the norm-relative error,
+#   sample  the values at SAMPLE fixed positions (seeded by the size) plus the position of max|ref|,
+#   blockmax  max|ref| over each of BLOCKS consecutive blocks of the flattened array: max|a| of every block must match
+#           within the elementwise tolerance (implied by |a - ref| <= tol * max|ref| everywhere), so a few wrong
+#           elements that change a block's extreme are caught wherever they are.
+SKETCH_K = 16
+SAMPLE = 24
+BLOCKS = 64
+_V_LEN = 3 + SKETCH_K + SAMPLE + 1          # norm, absmax, argmax, proj, sample (NaN padded)
+
+
+def _signs(n: int, j: int, device) -> torch.Tensor:
+    """+-1 vector j of length n from an integer hash of the index (the same on every device and torch version)."""
+    i = torch.arange(n, dtype=torch.int64, device=device)
+    h = (i * (2 * j + 0x9E3779B1) + 0x7F4A7C15 * (j + 1)) & 0xFFFFFFFF
+    h = h ^ (h >> 15)
+    h = (h * 0x2C1B3C6D) & 0xFFFFFFFF
+    h = h ^ (h >> 12)
+    return ((h >> 7) & 1).to(torch.float64) * 2.0 - 1.0
+
+
+def digest(a) -> str:
+    import hashlib
+    if isinstance(a, torch.Tensor):
+        a = a.detach().cpu().contiguous().numpy()
+    a = np.ascontiguousarray(a)
+    return hashlib.sha256(str(a.nbytes).encode() + a.tobytes()).hexdigest()
+
+
+def _projections(x: torch.Tensor) -> np.ndarray:
+    return np.array([float((x * _signs(x.numel(), j, x.device)).sum()) for j in range(SKETCH_K)])
+
+
+def _sample_index(n: int, argmax: int) -> np.ndarray:
+    idx = np.random.default_rng(n).choice(n, size=min(n, SAMPLE), replace=False)
+    return np.unique(np.append(idx, argmax))
+
+
+def _block_max(x: torch.Tensor) -> np.ndarray:
+    n = x.numel()
+    nb = min(BLOCKS, n)
+    blk = torch.arange(n, dtype=torch.int64, device=x.device) * nb // n
+    return torch.zeros(nb, dtype=x.dtype, device=x.device).scatter_reduce_(0, blk, x.abs(), "amax").cpu().numpy()
+
+
+def sketch(t: torch.Tensor) -> dict:
+    x = t.detach().reshape(-1).to(torch.float64)
+    rec = {"digest": digest(t), "shape": tuple(t.shape)}
+    if x.numel():
+        am = int(x.abs().argmax())
+        rec.update(norm=float(x.norm()), absmax=float(x.abs().max()), proj=_projections(x),
+                   sample=x[torch.from_numpy(_sample_index(x.numel(), am)).to(x.device)].cpu().numpy(), argmax=am,
+                   blockmax=_block_max(x))
+    return rec
+
+
+def sketch_rel_err(a: torch.Tensor, rec: dict) -> float:
+    """Estimate of ||a - ref|| / ||ref|| from the record of ref (0 if both are zero)."""
+    x = a.detach().reshape(-1).to(torch.float64)
+    d = _projections(x) - rec["proj"]
+    est = float(np.sqrt(np.mean(d * d)))
+    if rec["norm"] == 0.0:
+        return 0.0 if est == 0.0 and float(x.norm()) == 0.0 else float("inf")
+    return est / rec["norm"]
+
+
+def check_sketch(a: torch.Tensor, rec: dict, tol: float, name: str = "", elementwise: bool = True):
+    """`a` against the stored record: same shape, norm-relative error <= tol and, with `elementwise`, every sampled
+    element and the maximum of |a| over every block within tol * max|ref| (the tests' elementwise criterion on what is
+    stored of ref)."""
+    assert tuple(a.shape) == tuple(rec["shape"]), f"{name}: shape {tuple(a.shape)} vs {tuple(rec['shape'])}"
+    if a.numel() == 0:
+        return
+    e = sketch_rel_err(a, rec)
+    assert e <= tol, f"{name}: norm-relative error {e}"
+    x = a.detach().reshape(-1).to(torch.float64)
+    idx = _sample_index(x.numel(), int(rec["argmax"]))
+    worst = float(np.max(np.abs(x[torch.from_numpy(idx).to(x.device)].cpu().numpy() - rec["sample"][:idx.size])))
+    if elementwise and rec["absmax"] > 0:
+        assert worst <= tol * rec["absmax"], f"{name}: elementwise error {worst / rec['absmax']} of max|ref|"
+        bm = rec["blockmax"][:min(BLOCKS, x.numel())].astype(np.float64)
+        bworst = float(np.max(np.abs(_block_max(x) - bm)))
+        assert bworst <= tol * rec["absmax"], f"{name}: block maximum of |a| off by {bworst / rec['absmax']} of max|ref|"
+
+
+def save_records(path: str, records: dict):
+    """{case: {name: record or int}} -> one .npz, five arrays per case (names, digests, shapes, packed values,
+    block maxima in float32)."""
+    flat = {}
+    for case, arrays in records.items():
+        names, digests, shapes, vals, bmax = [], [], [], [], []
+        for name, rec in arrays.items():
+            if not isinstance(rec, dict):
+                flat[f"{case}/{name}"] = np.asarray(rec)
+                continue
+            v = np.full(_V_LEN, np.nan)
+            b = np.full(BLOCKS, np.nan, dtype=np.float32)
+            if "norm" in rec:
+                b[:rec["blockmax"].size] = rec["blockmax"]
+                v[:3] = rec["norm"], rec["absmax"], rec["argmax"]
+                v[3:3 + SKETCH_K] = rec["proj"]
+                v[3 + SKETCH_K:3 + SKETCH_K + rec["sample"].size] = rec["sample"]
+            names.append(name)
+            digests.append(rec["digest"])
+            shapes.append(",".join(str(int(d)) for d in rec.get("shape", ())) if "shape" in rec else "-")
+            vals.append(v)
+            bmax.append(b)
+        flat[f"{case}/names"] = np.array(names, dtype="S")
+        flat[f"{case}/digests"] = np.array(digests, dtype="S64")
+        flat[f"{case}/shapes"] = np.array(shapes, dtype="S")
+        flat[f"{case}/values"] = np.array(vals)
+        flat[f"{case}/blockmax"] = np.array(bmax)
+    np.savez_compressed(path, **flat)
+
+
+def load_records(path: str, case: str) -> dict:
+    out = {}
+    with np.load(path) as z:
+        keys = {k.split("/", 1)[1]: k for k in z.files if k.split("/", 1)[0] == case}
+        assert keys, f"no stored reference record for {case} in {os.path.basename(path)}"
+        for name, v, b in zip(z[keys["names"]], z[keys["values"]], z[keys["blockmax"]]):
+            out[name.decode()] = rec = {}
+            if not np.isnan(v[0]):
+                rec.update(norm=float(v[0]), absmax=float(v[1]), argmax=int(v[2]), proj=v[3:3 + SKETCH_K], sample=v[3 + SKETCH_K:],
+                           blockmax=b)
+        for name, d, sh in zip(z[keys["names"]], z[keys["digests"]], z[keys["shapes"]]):
+            out[name.decode()]["digest"] = d.decode()
+            if sh != b"-":
+                out[name.decode()]["shape"] = tuple(int(t) for t in sh.decode().split(",") if t)
+        for k, full in keys.items():
+            if k not in ("names", "digests", "shapes", "values", "blockmax"):
+                out[k] = z[full].item()
+    return out
+
+
 def make_inputs(scene_kind: str, n: int, W: int, H: int, mode: str, cam_k: int = 0, seed: int = 0,
                 opacity_mode: str = "random", device=None, **cam_kw):
     if scene_kind == "strands":

@@ -1,7 +1,7 @@
 """CPU tests: pin Oracle-B (oracle/gh_oracle.c) against
 
   * golden vectors produced by the REFERENCE ITSELF (its CUDA extension, built in place and run on a
-    B200 by tests/golden/make_golden.py): integer/bit state exact, floats to tolerance;
+    GPU by tests/golden/make_golden.py): integer/bit state exact, floats to tolerance;
   * golden vectors produced by the reference's own PYTHON restatement of stage 1
     (tests/golden/make_golden_pyref.py, run in the build container).
 """

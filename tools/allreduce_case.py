@@ -43,7 +43,7 @@ for name, mc in (("peer ld/st", False), ("multimem", True)):
     assert par.ok()
     if sweep:
         if mc:      # the NVLS path likes few requests in flight: sweep downwards too (grid smaller than the SM count)
-            grid = itertools.product((64, 128, 256, 512), (1, 2), (1, 2, 4, 8), (37, 74, 148, 1 << 20))
+            grid = itertools.product((64, 128, 256, 512), (1, 2), (1, 2, 4, 8), (33, 66, 132, 1 << 20))
         else:
             grid = itertools.product((128, 256, 512), (1, 2, 4), (1,), (1 << 20,))
         for th, cps, un, mx in grid:

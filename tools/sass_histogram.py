@@ -1,14 +1,14 @@
 """SASS opcode histogram of every kernel in the product library (no GPU needed):
-    python tools/sass_histogram.py [path/to/libgh_raster.so] > profiles/<tag>_sass_opcodes.txt
+    python tools/sass_histogram.py [path/to/libgh_raster.so] > <tag>_sass_opcodes.txt
 Counts are STATIC instruction counts per kernel (cuobjdump -sass); the columns are the mnemonics that identify the
-Blackwell-specific paths: packed FP32 (FFMA2 / FMUL2 / FADD2), LDGSTS (cp.async), UBLKCP + SYNCS (TMA bulk copy +
-mbarrier), REDG / RED (vector reductions to global memory), MATCH, UCGABAR_ARV / _WAIT (cluster barrier), LDGMC (multimem.ld_reduce, NVLS)."""
+Hopper paths: LDGSTS (cp.async), UBLKCP + SYNCS (TMA bulk copy + mbarrier), REDG / RED (vector reductions to global
+memory), MATCH, UCGABAR_ARV / _WAIT (cluster barrier), LDGMC (multimem.ld_reduce, NVLS)."""
 import collections, os, re, subprocess, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 lib = sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "gaussianhaircut_b200", "lib", "libgh_raster.so")
 sass = subprocess.run(["cuobjdump", "-sass", lib], capture_output=True, text=True, check=True).stdout
 names = subprocess.run(["cu++filt"], input="\n".join(re.findall(r"Function : (\S+)", sass)), capture_output=True, text=True).stdout.splitlines()
-COLS = ["FFMA2", "FMUL2", "FADD2", "FFMA", "MUFU", "LDGSTS", "UBLKCP", "SYNCS", "REDG", "RED", "ATOMG", "ATOMS", "MATCH", "SHFL",
+COLS = ["FFMA", "MUFU", "LDGSTS", "UBLKCP", "SYNCS", "REDG", "RED", "ATOMG", "ATOMS", "MATCH", "SHFL",
         "LDS", "STS", "LDG", "STG", "BAR", "UCGABAR*", "LDGMC", "DFMA", "FSEL"]
 kernels, cur = [], None
 for line in sass.splitlines():
@@ -18,7 +18,7 @@ for line in sass.splitlines():
     m = re.match(r"\s+/\*[0-9a-f]{4,}\*/\s+(?:@!?U?P\d+\s+)?([A-Z][A-Z0-9_]*)", line)
     if m and cur is not None:
         cur[m.group(1)] += 1; cur["_total"] += 1
-print(f"# {os.path.basename(lib)}: static SASS instruction counts per kernel (cuobjdump -sass, sm_100a)")
+print(f"# {os.path.basename(lib)}: static SASS instruction counts per kernel (cuobjdump -sass, sm_90a)")
 print(f"{'kernel':46s} {'total':>6s} " + " ".join(f"{c:>7s}" for c in COLS))
 for name, c in zip(names, kernels):
     short = re.sub(r"^.*?(gh_\w+).*$", r"\1", name)

@@ -298,7 +298,13 @@ __device__ __forceinline__ float gh_power(float dx, float dy, float ca, float cb
 }
 
 // ---- per-tile sort network (used by the forward blend CTA for its own list and by gh_segment_sort_kernel)
-#define GH_INKERNEL_SORT_MAX 2048u
+// Longest list the forward CTA sorts itself: 2 x 14 KB of keys + 6 KB of scratch keep the forward at 6 CTAs per SM.
+#ifndef GH_INKERNEL_SORT_MAX
+#define GH_INKERNEL_SORT_MAX 1792u
+#endif
+// GhBinWS::max_segments (R/768 + R/2048 + 2) bounds the segments of the long-list split only while every long list
+// has more than 1675 records: ceil(n/768) / n <= 1/768 + 1/2048 for n >= 1676.
+static_assert(GH_INKERNEL_SORT_MAX >= 1675u, "GhBinWS::max_segments assumes long lists of more than 1675 records");
 // Normalised bitonic network (every comparator puts the smaller key at the lower index), so
 // elements beyond n behave as +inf without being materialised: a comparator whose upper index
 // is >= n is simply skipped.
@@ -362,7 +368,7 @@ __device__ __forceinline__ void gh_bitonic_sort(KeyPtr keys, const uint32_t n, c
     }
 }
 
-// Sort up to 2048 records held in shared memory with an NT-thread CTA (NT = 128 or 256) in linear time:
+// Sort up to 2048 records (GH_INKERNEL_SORT_MAX in the forward CTA) held in shared memory with an NT-thread CTA (NT = 128 or 256) in linear time:
 // one MSD split of the records into 1024 sub-buckets by linearly quantised depth (order preserving),
 // then every thread insertion-sorts the records of its 1024 / NT consecutive sub-buckets (the range is
 // already partitioned, so records move only inside their sub-bucket); ranges longer than 32 records

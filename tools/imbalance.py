@@ -1,10 +1,14 @@
 """Measure the lock-step imbalance of the backward blend on a synthetic view (GPU tool).
 
-The backward kernel walks 8 per-block lists per warp in lock-step, so a warp spends
-max(len over its 8 blocks) steps per staged chunk.  This script rebuilds the per-block lists with
+The backward kernel walks the per-block lists of a warp in lock-step, so a warp spends
+max(len over its blocks) steps per staged window.  This script rebuilds the per-block lists with
 torch (exact alpha >= 1/255 test instead of the kernel's conservative span test, so it slightly
 under-counts) and prints   sum(len)/8   vs   sum(max len)   for the current block->warp mapping and
 for a per-tile mapping sorted by list length.
+
+Forward: the kernel's lanes own vertical pixel pairs and walk the union of the pair's two lists; a warp covers
+2 pair-rows x 16 columns (4 pixel rows) and a window holds 384 records.  The "forward PAIR" lines give its warp
+steps (the product: window 384, 2 row pairs x 16 cols); the one-pixel-per-lane lines are kept for comparison.
 
     python tools/imbalance.py [--strands 5000] [--res 1920x1080]
 """
@@ -48,18 +52,18 @@ def main():
     step = max(1, len(occupied) // args.max_tiles)
     sample = occupied[::step]
     tot_pairs = tot_cur = tot_sorted = tot_ideal = tot_pix = 0
-    CH = (256, 512, 1024, 4096)
+    CH = (256, 384, 512, 1024, 4096)
     bsteps = {k: [0, 0] for k in CH}      # backward: [current mapping, sorted mapping]
     fsteps = {k: 0 for k in CH}           # forward: warp = 2 pixel rows, per-pixel lists
     SHAPES = ((2, 16), (4, 8), (8, 4))
-    fshape = {(k, sh): 0 for k in (256, 512) for sh in SHAPES}
+    fshape = {(k, sh): 0 for k in (256, 384, 512) for sh in SHAPES}
     fpairs = 0
     inst_total = inst_contrib = inst_hit = inst_reached = 0
     ALT = ((4, 2), (2, 2), (2, 4), (8, 2), (4, 4))
     alt = {(bw, bh_, k): [0, 0] for (bw, bh_) in ALT for k in (256, 512)}
     alt_pix = {sh: 0 for sh in ALT}
     PSHAPES = ((2, 16), (4, 8))            # forward with a vertical pixel pair per lane: warp = row pairs x columns
-    fpair_steps = {(k, sh): 0 for k in (256, 512) for sh in PSHAPES}
+    fpair_steps = {(k, sh): 0 for k in (256, 384, 512) for sh in PSHAPES}
     fpair_entries = 0
     for t in sample:
         ty, tx = divmod(t, TX)
@@ -127,7 +131,7 @@ def main():
             bsteps[k][1] += int(cb[:, order].view(n, 4, 8).max(2).values.sum())
             cf = torch.nn.functional.pad(fh.int(), (0, 0, 0, n * k - L)).view(n, k, 8, 32).sum(1)   # [chunk, warp, lane]
             fsteps[k] += int(cf.max(2).values.sum())
-            if k in (256, 512):
+            if k in (256, 384, 512):
                 ph = fh.view(L, 8, 2, 16).any(2)                                   # [L, row pair, col]: union of the pair
                 if k == 256:
                     fpair_entries += int(ph.sum())
@@ -161,7 +165,8 @@ def main():
         print(f"forward  lock-step window {k:5d}: warp steps {fsteps[k]} (lane eff {fpairs / 32 / fsteps[k]:.3f})")
     print(f"forward pixel entries {fpairs}; pixel-PAIR entries {fpair_entries} ({fpair_entries / fpairs:.3f} of single)")
     for (k, sh), v in fpair_steps.items():
-        print(f"forward PAIR window {k} warp {sh[0]} row pairs x {sh[1]} cols: warp steps {v} (lane eff {fpair_entries / 32 / v:.3f})")
+        tag = "   <- product" if (k, sh) == (384, (2, 16)) else ""
+        print(f"forward PAIR window {k} warp {sh[0]} row pairs x {sh[1]} cols: warp steps {v} (lane eff {fpair_entries / 32 / v:.3f}){tag}")
     for (k, sh), v in fshape.items():
         print(f"forward window {k} warp shape {sh[0]}x{sh[1]}: warp steps {v} (lane eff {fpairs / 32 / v:.3f})")
 

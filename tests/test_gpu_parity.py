@@ -150,10 +150,14 @@ def test_parity_full_size(cuda_device, strands, mode, opm):
 
 
 def test_long_tile_lists(cuda_device):
-    """Tiles with > 2048 instances take the large shared-memory sort; > 24576 the in-place one."""
+    """Tiles with more than GH_INKERNEL_SORT_MAX (1792) instances are split into depth segments of ~768 records
+    (gh_tile_split_long_kernel) and each segment is sorted by gh_segment_sort_kernel -- in shared memory when it
+    holds at most 1792 records.  This scene's lists are tens of thousands of records long, so the split and the
+    shared-memory segment sort do most of the work; a segment longer than 1792 records (sorted in place in global
+    memory) is what tests/test_gpu_blend_replay.py::test_equal_depths reaches."""
     o = _run("long-lists", cuda_device)
     rg = o["mine_state"]["ranges"].view(np.uint32)
-    assert (rg[:, 1] - rg[:, 0]).max() > 24576, "test scene no longer reaches the in-place sort path"
+    assert (rg[:, 1] - rg[:, 0]).max() > 24576, "test scene no longer has lists of many segments"
     _check_binning(o)
     _check_image(o)
     _check_grads(o)
@@ -179,14 +183,15 @@ def _two_tile_scene(n_first, n_second, W=32, H=16):
     return scene, synth.make_camera(0, W, H)
 
 
-TWO_TILE_CASES = [(1, 2048), (1, 2047), (2, 2048), (1, 2046), (3, 2049)]
+TWO_TILE_CASES = [(1, 1792), (1, 1791), (2, 1792), (1, 1790), (3, 1793)]
 
 
 @pytest.mark.parametrize("n_first,n_second", TWO_TILE_CASES)
 def test_in_cta_sort_boundary(cuda_device, n_first, n_second):
-    """Buckets of 2046..2049 records starting at odd / even record indices: the widened TMA load of the
-    bucket, its fallback loop (bucket would not fit after widening) and the hand-over to the long-list
-    kernels at 2049 -- sort order and everything downstream against the reference build."""
+    """Buckets of 1790..1793 records starting at odd / even record indices, around GH_INKERNEL_SORT_MAX (1792): the
+    widened TMA load of the bucket, its fallback loop (1792 records from an odd index do not fit after widening) and
+    the hand-over to the long-list kernels at 1793 -- sort order and everything downstream against the reference
+    build."""
     o = _run(f"two-tiles-{n_first}-{n_second}", cuda_device)
     rg = o["mine_state"]["ranges"].view(np.uint32)
     assert int(rg[0, 1] - rg[0, 0]) == n_first and int(rg[1, 0]) == n_first and int(rg[1, 1] - rg[1, 0]) == n_second

@@ -101,6 +101,8 @@ SIGNATURES = {
         _p, _p, _p, _p, _p, _p,              # d_xyz d_scaling d_rotation d_dirs d_features_dc d_features_rest
         _p, _p, _p, _p, _p,                  # d_opacity d_label d_orient_conf d_means2D d_camera
         _p, _p, _p]),                        # nan_flag workspace stream
+    "gh_strand_midpoints": (_i, [_i, _i, _p, _p, _p, _p]),          # S L origins dirs xyz stream
+    "gh_strand_backward": (_i, [_i, _i, _p, _p, _p, _p]),           # S L d_xyz d_dirs nan_flag stream
     "gh_densify_classify": (_i, [_i, _p, _p, _p, _p, _f, _f, _f, _f, _p, _p]),
     "gh_densify_scatter": (_i, [_i, _i, _p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _p, _p, _i, _i, _i, _p, _i, _p]),
     "gh_debug_export": (_i, [_i, _i, _i, _ll, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),

@@ -69,7 +69,8 @@ __device__ __forceinline__ void gh_rest_store(const float* s_rest, float* __rest
 // per-tile instance histogram -- the conic, mean and opacity are still in registers, so the rasterizer's own
 // preprocess launch (and its re-read of 28 bytes per Gaussian) disappears from a fused render.  Same device functions
 // as gh_preprocess_kernel (gh_common.cuh), hence bit-identical radii / records / keys.
-template <bool BIN>
+// STRAND: Gaussian i is a polyline segment whose scales and rotation come from dirs[i] (gh_proj_geometry).
+template <bool BIN, bool STRAND>
 __global__ void __launch_bounds__(GH_PJ_THREADS)
 gh_project_forward_kernel(GhProjArgs A, float* __restrict__ means2D, float* __restrict__ colors,
                           float* __restrict__ opac_out, float* __restrict__ conic_out, float* __restrict__ cov3D_out,
@@ -85,7 +86,7 @@ gh_project_forward_kernel(GhProjArgs A, float* __restrict__ means2D, float* __re
     int rect_minx = 0, rect_miny = 0, rect_maxx = 0, rect_maxy = 0;
     if (i < A.P) {
         GhProjOut o;
-        gh_project_forward_one(A, i, s_rest + threadIdx.x * GH_PJ_REST, cov3D_out != nullptr, o);
+        gh_project_forward_one<STRAND>(A, i, s_rest + threadIdx.x * GH_PJ_REST, cov3D_out != nullptr, o);
         means2D[3 * (size_t)i] = o.m2[0]; means2D[3 * (size_t)i + 1] = o.m2[1]; means2D[3 * (size_t)i + 2] = o.m2[2];
         conic_out[3 * (size_t)i] = o.conic[0]; conic_out[3 * (size_t)i + 1] = o.conic[1]; conic_out[3 * (size_t)i + 2] = o.conic[2];
         mask_out[i] = o.visible ? 1 : 0;
@@ -122,6 +123,8 @@ gh_project_forward_kernel(GhProjArgs A, float* __restrict__ means2D, float* __re
 // dL_dconic (P,4) = (d/da, HALF d/db, unused, d/dc), dL_dcolor (P,10), dL_dopacity (P)), or -- when acc16 is
 // given -- the blend backward's 64-byte accumulation records themselves (colors 0..9, mean2D x y, conic x y w,
 // opacity), which skips the unpack kernel and its round trip through HBM.
+// STRAND: the scale and rotation gradients are folded into d_dirs in registers; d_scaling / d_rotation are not written.
+template <bool STRAND>
 __global__ void __launch_bounds__(GH_PJ_THREADS)
 gh_project_backward_kernel(GhProjArgs A, const unsigned char* __restrict__ mask,
                            const float* __restrict__ acc16,
@@ -177,13 +180,15 @@ gh_project_backward_kernel(GhProjArgs A, const unsigned char* __restrict__ mask,
 #pragma unroll
                 for (int k = 0; k < GH_NUM_CHANNELS / 2; k++) { const float2 v = cr[k]; gi.color[2 * k] = v.x; gi.color[2 * k + 1] = v.y; }
             }
-            gh_project_backward_one(A, i, s_rest + threadIdx.x * GH_PJ_REST, gi, go, cam);
+            gh_project_backward_one<STRAND>(A, i, s_rest + threadIdx.x * GH_PJ_REST, gi, go, cam);
         }
         // every row of every per-Gaussian gradient is written (zeros for culled Gaussians)
         if (d_mean2D_out) { d_mean2D_out[3 * (size_t)i] = gi.m2x; d_mean2D_out[3 * (size_t)i + 1] = gi.m2y; d_mean2D_out[3 * (size_t)i + 2] = 0.f; }
         d_xyz[3 * (size_t)i] = go.xyz[0]; d_xyz[3 * (size_t)i + 1] = go.xyz[1]; d_xyz[3 * (size_t)i + 2] = go.xyz[2];
-        d_scaling[3 * (size_t)i] = go.scaling[0]; d_scaling[3 * (size_t)i + 1] = go.scaling[1]; d_scaling[3 * (size_t)i + 2] = go.scaling[2];
-        reinterpret_cast<float4*>(d_rotation)[i] = make_float4(go.rotation[0], go.rotation[1], go.rotation[2], go.rotation[3]);
+        if (!STRAND) {
+            d_scaling[3 * (size_t)i] = go.scaling[0]; d_scaling[3 * (size_t)i + 1] = go.scaling[1]; d_scaling[3 * (size_t)i + 2] = go.scaling[2];
+            reinterpret_cast<float4*>(d_rotation)[i] = make_float4(go.rotation[0], go.rotation[1], go.rotation[2], go.rotation[3]);
+        }
         if (d_dirs) { d_dirs[3 * (size_t)i] = go.dirs[0]; d_dirs[3 * (size_t)i + 1] = go.dirs[1]; d_dirs[3 * (size_t)i + 2] = go.dirs[2]; }
         d_fdc[3 * (size_t)i] = go.f_dc[0]; d_fdc[3 * (size_t)i + 1] = go.f_dc[1]; d_fdc[3 * (size_t)i + 2] = go.f_dc[2];
         if (d_opacity) d_opacity[i] = go.opacity;
@@ -262,11 +267,17 @@ gh_project_backward_kernel(GhProjArgs A, const unsigned char* __restrict__ mask,
     }
 }
 
-int gh_proj_check(GhProjArgs& A, const char* who)
+int gh_proj_check(GhProjArgs& A, const char* who, bool strand)
 {
     char msg[160];
     if (A.P <= 0 || A.W <= 0 || A.H <= 0) { snprintf(msg, sizeof msg, "%s: P, width, height must be positive", who); return gh_set_error(GH_E_INVALID_ARG, msg); }
-    if (!A.xyz || !A.scaling || !A.rotation || !A.f_dc || !A.V || !A.Pm || !A.campos) { snprintf(msg, sizeof msg, "%s: missing mandatory pointer", who); return gh_set_error(GH_E_INVALID_ARG, msg); }
+    if (strand) {
+        if (A.rotation) { snprintf(msg, sizeof msg, "%s: strand mode derives the rotation from dirs, rotation must be NULL", who); return gh_set_error(GH_E_INVALID_ARG, msg); }
+        if (!A.dirs) { snprintf(msg, sizeof msg, "%s: strand mode needs dirs (the segment vectors)", who); return gh_set_error(GH_E_INVALID_ARG, msg); }
+        if (!A.scaling) { snprintf(msg, sizeof msg, "%s: strand mode needs scaling = the strand thickness (one device float)", who); return gh_set_error(GH_E_INVALID_ARG, msg); }
+        if (A.scale_act != 0 || A.dir_mode != 1) { snprintf(msg, sizeof msg, "%s: strand mode needs scale activation 0 and direction mode 1", who); return gh_set_error(GH_E_INVALID_ARG, msg); }
+    }
+    if (!A.xyz || !A.scaling || (!strand && !A.rotation) || !A.f_dc || !A.V || !A.Pm || !A.campos) { snprintf(msg, sizeof msg, "%s: missing mandatory pointer", who); return gh_set_error(GH_E_INVALID_ARG, msg); }
     if (A.sh_degree < 0 || A.sh_degree > 3) { snprintf(msg, sizeof msg, "%s: sh_degree must be 0..3", who); return gh_set_error(GH_E_INVALID_ARG, msg); }
     if (A.sh_degree > 0 && !A.f_rest) { snprintf(msg, sizeof msg, "%s: features_rest required for sh_degree > 0", who); return gh_set_error(GH_E_INVALID_ARG, msg); }
     if ((size_t)A.rotation & 15) { snprintf(msg, sizeof msg, "%s: rotation must be 16-byte aligned", who); return gh_set_error(GH_E_INVALID_ARG, msg); }
@@ -293,6 +304,9 @@ GhProjArgs gh_proj_args(int P, int width, int height, const float* xyz, const fl
     return A;
 }
 
+// flag bit 10: the strand instantiation (Gaussian i = segment i of a polyline, geometry derived from dirs[i])
+bool gh_proj_strand(unsigned int flags) { return (flags >> 10) & 1u; }
+
 }  // namespace
 
 extern "C" int gh_project_workspace_size(int P, size_t* bytes)
@@ -318,11 +332,13 @@ extern "C" int gh_project_forward(
     gh_clear_error();
     GhProjArgs A = gh_proj_args(P, width, height, xyz, scaling, rotation, dirs, features_dc, features_rest, opacity, label,
                                 orient_conf, viewmatrix, projmatrix, campos, tan_fovx, tan_fovy, scale_modifier, sh_degree, flags, det_eps);
-    const int rc = gh_proj_check(A, "gh_project_forward");
+    const bool strand = gh_proj_strand(flags);
+    const int rc = gh_proj_check(A, "gh_project_forward", strand);
     if (rc != GH_OK) return rc;
     if (!means2D || !colors || !opacities || !conic || !visible) return gh_set_error(GH_E_INVALID_ARG, "gh_project_forward: missing output pointer");
     if ((size_t)colors & 7) return gh_set_error(GH_E_INVALID_ARG, "gh_project_forward: colors must be 8-byte aligned");
-    gh_project_forward_kernel<false><<<(P + GH_PJ_THREADS - 1) / GH_PJ_THREADS, GH_PJ_THREADS, 0, stream>>>(
+    auto kernel = strand ? gh_project_forward_kernel<false, true> : gh_project_forward_kernel<false, false>;
+    kernel<<<(P + GH_PJ_THREADS - 1) / GH_PJ_THREADS, GH_PJ_THREADS, 0, stream>>>(
         A, means2D, colors, opacities, conic, cov3D, visible, nullptr, nullptr, nullptr, nullptr, 0, 0);
     gh_count_launches(1);
     const cudaError_t e = cudaGetLastError();
@@ -347,7 +363,8 @@ extern "C" int gh_project_forward_binned(
     gh_clear_error();
     GhProjArgs A = gh_proj_args(P, width, height, xyz, scaling, rotation, dirs, features_dc, features_rest, opacity, label,
                                 orient_conf, viewmatrix, projmatrix, campos, tan_fovx, tan_fovy, scale_modifier, sh_degree, flags, det_eps);
-    const int rc = gh_proj_check(A, "gh_project_forward_binned");
+    const bool strand = gh_proj_strand(flags);
+    const int rc = gh_proj_check(A, "gh_project_forward_binned", strand);
     if (rc != GH_OK) return rc;
     if (!means2D || !colors || !opacities || !conic || !visible || !radii || !geom_buffer || !img_buffer || !num_rendered)
         return gh_set_error(GH_E_INVALID_ARG, "gh_project_forward_binned: missing output pointer");
@@ -361,7 +378,8 @@ extern "C" int gh_project_forward_binned(
     // ctrl + tile histogram are contiguous: one memset
     cudaError_t e = cudaMemsetAsync(img.ctrl, 0, 256 + gh_align_up((size_t)T * 4, 256), stream);
     if (e != cudaSuccess) return gh_set_error(GH_E_CUDA, "gh_project_forward_binned: memset(tile histogram) failed");
-    gh_project_forward_kernel<true><<<(P + GH_PJ_THREADS - 1) / GH_PJ_THREADS, GH_PJ_THREADS, 0, stream>>>(
+    auto kernel = strand ? gh_project_forward_kernel<true, true> : gh_project_forward_kernel<true, false>;
+    kernel<<<(P + GH_PJ_THREADS - 1) / GH_PJ_THREADS, GH_PJ_THREADS, 0, stream>>>(
         A, means2D, colors, opacities, conic, cov3D, visible, radii, geom.geo, geom.depth, img.tile_count, gx, gy);
     gh_launch_tile_scan(T, img, stream);
     gh_count_launches(2);
@@ -392,9 +410,14 @@ extern "C" int gh_project_backward(
     gh_clear_error();
     GhProjArgs A = gh_proj_args(P, width, height, xyz, scaling, rotation, dirs, features_dc, features_rest, opacity, label,
                                 orient_conf, viewmatrix, projmatrix, campos, tan_fovx, tan_fovy, scale_modifier, sh_degree, flags, det_eps);
-    const int rc = gh_proj_check(A, "gh_project_backward");
+    const bool strand = gh_proj_strand(flags);
+    const int rc = gh_proj_check(A, "gh_project_backward", strand);
     if (rc != GH_OK) return rc;
-    if (!visible || !d_xyz || !d_scaling || !d_rotation || !d_features_dc || !d_features_rest)
+    if (strand && (d_scaling || d_rotation))
+        return gh_set_error(GH_E_INVALID_ARG, "gh_project_backward: strand mode folds scale and rotation gradients into d_dirs, d_scaling / d_rotation must be NULL");
+    if (strand && !d_dirs)
+        return gh_set_error(GH_E_INVALID_ARG, "gh_project_backward: strand mode needs d_dirs");
+    if (!visible || !d_xyz || (!strand && (!d_scaling || !d_rotation)) || !d_features_dc || !d_features_rest)
         return gh_set_error(GH_E_INVALID_ARG, "gh_project_backward: missing mandatory pointer");
     if (geom_buffer == nullptr && (!dL_dmeans2D || !dL_dconic || !dL_dcolors || !dL_dopacity))
         return gh_set_error(GH_E_INVALID_ARG, "gh_project_backward: pass the geometry workspace of gh_backward or the four incoming gradients");
@@ -411,7 +434,8 @@ extern "C" int gh_project_backward(
         if (cudaMemsetAsync(ticket, 0, sizeof(unsigned int), stream) != cudaSuccess)
             return gh_set_error(GH_E_CUDA, "gh_project_backward: memset(ticket) failed");
     }
-    gh_project_backward_kernel<<<(P + GH_PJ_THREADS - 1) / GH_PJ_THREADS, GH_PJ_THREADS, 0, stream>>>(
+    auto kernel = strand ? gh_project_backward_kernel<true> : gh_project_backward_kernel<false>;
+    kernel<<<(P + GH_PJ_THREADS - 1) / GH_PJ_THREADS, GH_PJ_THREADS, 0, stream>>>(
         A, visible, acc16, dL_dmeans2D, dL_dconic, dL_dcolors, dL_dopacity,
         d_xyz, d_scaling, d_rotation, d_dirs, d_features_dc, d_features_rest, d_opacity, d_label, d_orient_conf,
         d_means2D, partial, ticket, d_camera, nan_flag);

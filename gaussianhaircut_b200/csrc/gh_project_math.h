@@ -131,15 +131,30 @@ struct GhProjGeo {
     float a, b, c;       // cov2D incl. the 0.3 low-pass
 };
 
+// STRAND: the Gaussian is segment i of a polyline (gaussian_model_strands.py:435-454).  Its scales and rotation are
+// derived in registers from the segment vector d = dirs[i]: scales (|d|/2, scale, scale) with the strand thickness
+// `scale` = scaling[0] (one float for the whole model), rotation parallel_transport(e_x, d) = (1 + b.x, 0, -b.z, b.y)
+// with b = d / max(|d|, 1e-12) (general_utils.py:150-160).  `rotation` is not read.
+template <bool STRAND = false>
 GH_HD void gh_proj_geometry(const GhProjArgs& A, int i, GhProjGeo& g) {
     g.x[0] = A.xyz[3 * (size_t)i]; g.x[1] = A.xyz[3 * (size_t)i + 1]; g.x[2] = A.xyz[3 * (size_t)i + 2];
+    float q0, q1, q2, q3;
+    if constexpr (STRAND) {
+        const float dx = A.dirs[3 * (size_t)i], dy = A.dirs[3 * (size_t)i + 1], dz = A.dirs[3 * (size_t)i + 2];
+        const float dn = sqrtf(dx * dx + dy * dy + dz * dz);
+        const float th = GH_LDG(A.scaling) * A.mod;
+        g.s[0] = (dn * 0.5f) * A.mod; g.s[1] = th; g.s[2] = th;
+        const float ib = 1.0f / fmaxf(dn, 1e-12f);
+        q0 = 1.0f + dx * ib; q1 = 0.f; q2 = -(dz * ib); q3 = dy * ib;
+    } else {
 #pragma unroll
-    for (int k = 0; k < 3; k++) {
-        const float v = A.scaling[3 * (size_t)i + k];
-        g.s[k] = (A.scale_act == 1 ? expf(v) : v) * A.mod;
+        for (int k = 0; k < 3; k++) {
+            const float v = A.scaling[3 * (size_t)i + k];
+            g.s[k] = (A.scale_act == 1 ? expf(v) : v) * A.mod;
+        }
+        const float* qp = A.rotation + 4 * (size_t)i;
+        q0 = qp[0]; q1 = qp[1]; q2 = qp[2]; q3 = qp[3];
     }
-    const float* qp = A.rotation + 4 * (size_t)i;
-    const float q0 = qp[0], q1 = qp[1], q2 = qp[2], q3 = qp[3];
     g.qlen = sqrtf(q0 * q0 + q1 * q1 + q2 * q2 + q3 * q3);
     const float il = 1.0f / g.qlen;
     const float r = q0 * il, x = q1 * il, y = q2 * il, z = q3 * il;
@@ -211,9 +226,10 @@ struct GhProjOut {
 };
 
 // One Gaussian, forward.  `rest` = this Gaussian's f_rest row (45 floats, coefficient-major, RGB-minor).
+template <bool STRAND = false>
 GH_HD void gh_project_forward_one(const GhProjArgs& A, int i, const float* rest, bool want_cov3D, GhProjOut& o) {
     GhProjGeo g;
-    gh_proj_geometry(A, i, g);
+    gh_proj_geometry<STRAND>(A, i, g);
     const float* Pm = A.Pm;
     float h[4];
 #pragma unroll
@@ -291,10 +307,13 @@ struct GhProjGradOut {
 //   [0..11]  dL/dV[i][j]  (i = 0..3 rows, j = 0..2)          index 3*i + j
 //   [12..23] dL/dPm[i][c] (i = 0..3 rows, c in {0, 1, 3})    index 12 + 3*i + {0, 1, 2}
 //   [24..26] dL/dcampos, [27..28] dL/dtan(fovx/2), dL/dtan(fovy/2)
+// STRAND: the scale and rotation gradients are folded into go.dirs (the segment vector's direct term) and
+// go.scaling / go.rotation come back as zeros; go.xyz is the gradient w.r.t. the segment's midpoint.
+template <bool STRAND = false>
 GH_HD void gh_project_backward_one(const GhProjArgs& A, int i, const float* rest, const GhProjGradIn& gi,
                                    GhProjGradOut& go, float* cam) {
     GhProjGeo g;
-    gh_proj_geometry(A, i, g);
+    gh_proj_geometry<STRAND>(A, i, g);
     const float* V = A.V;
     const float* Pm = A.Pm;
     float dx[3] = {0.f, 0.f, 0.f}, ds[3] = {0.f, 0.f, 0.f};
@@ -478,4 +497,21 @@ GH_HD void gh_project_backward_one(const GhProjArgs& A, int i, const float* rest
 #pragma unroll
     for (int k = 0; k < 3; k++) go.scaling[k] = (A.scale_act == 1) ? ds[k] * g.s[k] : ds[k] * A.mod;
     go.xyz[0] = dx[0]; go.xyz[1] = dx[1]; go.xyz[2] = dx[2];
+    if constexpr (STRAND) {
+        // q = (1 + b.x, 0, -b.z, b.y): dL/db from the raw-quaternion gradient, through b = d / max(|d|, 1e-12);
+        // scale 0 = |d| / 2 adds 0.5 dL/ds0 d / |d|.  The thickness is not a parameter: its gradient is dropped.
+        const float n0 = A.dirs[3 * (size_t)i], n1 = A.dirs[3 * (size_t)i + 1], n2 = A.dirs[3 * (size_t)i + 2];
+        const float dl = fmaxf(sqrtf(n0 * n0 + n1 * n1 + n2 * n2), 1e-12f);
+        const float b0 = n0 / dl, b1 = n1 / dl, b2 = n2 / dl;
+        const float gb0 = go.rotation[0], gb1 = go.rotation[3], gb2 = -go.rotation[2];
+        const float dot = b0 * gb0 + b1 * gb1 + b2 * gb2;
+        const float hs = 0.5f * go.scaling[0];
+        go.dirs[0] += (gb0 - b0 * dot) / dl + hs * b0;
+        go.dirs[1] += (gb1 - b1 * dot) / dl + hs * b1;
+        go.dirs[2] += (gb2 - b2 * dot) / dl + hs * b2;
+#pragma unroll
+        for (int k = 0; k < 3; k++) go.scaling[k] = 0.f;
+#pragma unroll
+        for (int k = 0; k < 4; k++) go.rotation[k] = 0.f;
+    }
 }

@@ -29,11 +29,14 @@ GAUSSIAN_MODEL = dict(scale_act=1, opacity_act=1, label_act=1, conf_act=1, dir_m
 HAIR_MODEL = dict(scale_act=0, opacity_act=2, label_act=2, conf_act=1, dir_mode=1, det_eps=1e-7)         # gaussian_model_latent_strands.py
 # the frozen head Gaussians inside render_hair(): activated scales / opacities, label = dir2D = confidence = 0
 HEAD_PRECOMP = dict(scale_act=0, opacity_act=0, label_act=3, conf_act=3, dir_mode=2, det_eps=1e-12)
+# GaussianModelCurves (gaussian_model_strands.py) rendered from its polylines: HAIR_MODEL semantics, but every Gaussian is
+# a segment whose scales / rotation the kernels derive from dirs[i]; `scaling` is the (1,) strand thickness, no rotation
+HAIR_STRANDS = dict(HAIR_MODEL, strands=1)
 
 
 def encode_flags(cfg: Dict[str, object]) -> int:
     return (int(cfg["scale_act"]) & 3) | ((int(cfg["opacity_act"]) & 3) << 2) | ((int(cfg["label_act"]) & 3) << 4) | \
-           ((int(cfg["conf_act"]) & 3) << 6) | ((int(cfg["dir_mode"]) & 3) << 8)
+           ((int(cfg["conf_act"]) & 3) << 6) | ((int(cfg["dir_mode"]) & 3) << 8) | ((int(cfg.get("strands", 0)) & 1) << 10)
 
 
 def _ptr(t: Optional[torch.Tensor]):
@@ -92,7 +95,13 @@ def pack_inputs(xyz, scaling, rotation, dirs, f_dc, f_rest, opacity, label, conf
     pi.mod, pi.sh_degree = float(scaling_modifier), int(sh_degree)
     pi.flags, pi.det_eps = encode_flags(cfg), float(cfg["det_eps"])
     n = pi.P
-    for name, t, per in (("scaling", pi.scaling, 3), ("rotation", pi.rotation, 4), ("features_dc", pi.f_dc, 3)):
+    if cfg.get("strands", 0):
+        if pi.scaling is None or pi.scaling.numel() != 1 or pi.rotation is not None:
+            raise RuntimeError("projection: strand mode takes the strand thickness as a (1,) 'scaling' tensor and no rotation")
+        per_row = (("dirs", pi.dirs, 3), ("features_dc", pi.f_dc, 3), ("orient_conf", pi.conf, 1))
+    else:
+        per_row = (("scaling", pi.scaling, 3), ("rotation", pi.rotation, 4), ("features_dc", pi.f_dc, 3))
+    for name, t, per in per_row:
         if t is None or t.numel() != n * per:
             raise RuntimeError(f"projection: '{name}' must have {per} floats per Gaussian")
     if pi.sh_degree > 0 and (pi.f_rest is None or pi.f_rest.numel() != n * 45):
@@ -220,6 +229,9 @@ def project_backward(pi: ProjectionInputs, visible: torch.Tensor, geom_buffer: O
     lib = _capi.load()
     dev, P = pi.device, pi.P
     f = dict(dtype=torch.float32, device=dev)
+    strand = bool(pi.flags >> 10 & 1)
+    if strand and _GRAD_ARENA["storage"] is not None:
+        raise RuntimeError("projection: the strand model has no gradient-arena layout; remove the arena (set_gradient_arena(None))")
     if _GRAD_ARENA["storage"] is not None:
         a = carve_grad_arena(_GRAD_ARENA["storage"], P, with_dirs=pi.dirs is not None)
         _GRAD_ARENA["last"] = P
@@ -231,7 +243,8 @@ def project_backward(pi: ProjectionInputs, visible: torch.Tensor, geom_buffer: O
         del a
     else:
         f32 = torch.float32
-        g = {"xyz": empty_rows(P, (3,), f32, dev), "scaling": empty_rows(P, (3,), f32, dev), "rotation": empty_rows(P, (4,), f32, dev),
+        g = {"xyz": empty_rows(P, (3,), f32, dev),
+             "scaling": None if strand else empty_rows(P, (3,), f32, dev), "rotation": None if strand else empty_rows(P, (4,), f32, dev),
              "dirs": empty_rows(P, (3,), f32, dev) if pi.dirs is not None else None,
              "f_dc": empty_rows(P, (1, 3), f32, dev), "f_rest": empty_rows(P, (15, 3), f32, dev),
              "opacity": empty_rows(P, (1,), f32, dev) if pi.opacity is not None else None,
@@ -254,3 +267,30 @@ def project_backward(pi: ProjectionInputs, visible: torch.Tensor, geom_buffer: O
         g["viewmatrix"], g["projmatrix"] = cam[0:16].view(4, 4), cam[16:32].view(4, 4)
         g["campos"], g["tanfov"] = cam[32:35], cam[35:37]
     return g
+
+
+# ------------------------------------------------------------------------------------------------- strand geometry
+def strand_midpoints(origins: torch.Tensor, dirs: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
+    """Segment midpoints of S polylines (gh_strand_midpoints): origins (S,1,3), dirs (S,L,3) -> `out` (S*L,3), a
+    contiguous float32 buffer (e.g. a row block of a larger means3D buffer); what initialize_gaussians_hair() computes
+    as `_xyz` (gaussian_model_strands.py:436-438), up to the summation order of the scan."""
+    lib = _capi.load()
+    S, L = int(dirs.shape[0]), int(dirs.shape[1])
+    dev = out.device
+    o = _f32(origins, "pts_origins", dev)
+    d = _f32(dirs, "dirs", dev)
+    if not out.is_contiguous() or out.shape != (S * L, 3):
+        raise RuntimeError(f"strand_midpoints: 'out' must be a contiguous ({S * L}, 3) tensor")
+    with torch.cuda.device(dev):
+        _capi.check(lib.gh_strand_midpoints(S, L, _ptr(o), _ptr(d), _ptr(out), _stream(dev)))
+    return out
+
+
+def strand_backward(S: int, L: int, d_xyz: torch.Tensor, d_dirs: torch.Tensor, nan_flag: Optional[torch.Tensor] = None):
+    """gh_strand_backward: d_dirs (S*L,3), holding the direct terms of the strand-mode projection backward, becomes
+    dL/d_dirs IN PLACE (the midpoint gradients d_xyz chained through the cumulative sum); returns it as (S,L,3)."""
+    lib = _capi.load()
+    dev = d_dirs.device
+    with torch.cuda.device(dev):
+        _capi.check(lib.gh_strand_backward(S, L, _ptr(d_xyz), _ptr(d_dirs), _ptr(nan_flag), _stream(dev)))
+    return d_dirs.view(S, L, 3)

@@ -26,7 +26,7 @@ import torch.nn.functional as F
 from . import _C, projection
 from ._alloc import empty_rows
 
-__all__ = ["render", "render_hair", "render_raw", "set_nan_flag"]
+__all__ = ["render", "render_hair", "render_hair_strands", "render_raw", "set_nan_flag"]
 
 _EMPTY = torch.Tensor([])
 
@@ -70,17 +70,29 @@ class _FusedRender(torch.autograd.Function):
     """(xyz, scaling, rotation, dirs, f_dc, f_rest, opacity, label, conf, viewspace, viewmatrix, projmatrix, campos, tanfov,
     static) -> (raw 10-channel image, radii).  `viewspace` is a (P,3) leaf: its storage receives the NDC means and its
     gradient the rasterizer's dL/dmeans2D (what `add_densification_stats` reads).  `static`: dict of non-tensors + the
-    frozen head block of render_hair()."""
+    frozen head block of render_hair().
+    Strand models (render_hair_strands, static["strands"] = polyline origins): xyz is None, `dirs` is the (S,L,3) segment
+    vector parameter and `scaling` the (1,) strand thickness; the segment midpoints are computed into the means3D rows
+    of this model and kept for the backward, which returns the gradient of `dirs` (S,L,3)."""
 
     @staticmethod
     def forward(ctx, xyz, scaling, rotation, dirs, f_dc, f_rest, opacity, label, conf, viewspace, viewmatrix, projmatrix,
                 campos, tanfov, static):
         st = static
-        dev = xyz.device
+        dev = viewspace.device
         head = st.get("head")
         n_head = 0 if head is None else int(head["xyz"].shape[0])
-        P_own = int(xyz.shape[0])
+        strands = st.get("strands")
+        P_own = int(dirs.shape[0] * dirs.shape[1]) if strands is not None else int(xyz.shape[0])
         P = n_head + P_own
+        means3D = None
+        if strands is not None:
+            # segment midpoints straight into this model's rows of the means3D buffer (behind the head rows: no cat)
+            means3D = empty_rows(P, (3,), torch.float32, dev)
+            if n_head > 0:
+                means3D[:n_head].copy_(head["xyz"])
+            xyz = projection.strand_midpoints(strands["origins"], dirs, out=means3D[n_head:])
+            dirs = dirs.reshape(P_own, 3)
         pi = projection.pack_inputs(xyz, scaling, rotation, dirs, f_dc, f_rest, opacity, label, conf, viewmatrix, projmatrix,
                                     campos, st["tanx"], st["tany"], st["W"], st["H"], st["sh_degree"], st["mod"], st["cfg"])
         bg = st["bg"]
@@ -104,7 +116,8 @@ class _FusedRender(torch.autograd.Function):
             sl = lambda a, b: {k: (v[a:b] if v is not None else None) for k, v in out.items()}  # noqa: E731
             projection.project_forward(hp, out=sl(0, n_head))
             projection.project_forward(pi, out=sl(n_head, P))
-            means3D = torch.cat([hp.xyz, pi.xyz], dim=0)
+            if means3D is None:
+                means3D = torch.cat([hp.xyz, pi.xyz], dim=0)
         R, color, radii, geom, binning, img = _C.rasterize_gaussians(
             bg, means3D, _EMPTY, out["colors"], out["opacity"], _EMPTY, _EMPTY, st["mod"], _EMPTY, out["conic"],
             pi.V, pi.Pm, st["tanx"], st["tany"], st["H"], st["W"], _EMPTY, st["sh_degree"], pi.campos,
@@ -143,6 +156,10 @@ class _FusedRender(torch.autograd.Function):
                                                  dL_dcolors=g_col[:n_head], dL_dopacity=g_op[:n_head], camera_grads=True)
                 for k in ("viewmatrix", "projmatrix", "campos", "tanfov"):
                     g[k] = g[k] + gh[k]
+        strands = st.get("strands")
+        if strands is not None:
+            # the per-segment midpoint gradients, chained through the cumulative sum into the segment vectors
+            g["dirs"] = projection.strand_backward(strands["S"], strands["L"], g["xyz"], g["dirs"], nan_flag=_NAN_FLAG["t"])
         pick = lambda k, idx: g.get(k) if need[idx] else None  # noqa: E731   (autograd rejects gradients for non-Variable inputs)
         return (pick("xyz", 0), pick("scaling", 1), pick("rotation", 2), pick("dirs", 3), pick("f_dc", 4), pick("f_rest", 5),
                 pick("opacity", 6), pick("label", 7), pick("conf", 8), g_view if need[9] else None,
@@ -228,4 +245,49 @@ def render_hair(viewpoint_camera, pc, pc_hair, pipe, bg_color: torch.Tensor, sca
         pc_hair.get_xyz, pc_hair.get_scaling, pc_hair._rotation, pc_hair._dir, pc_hair._features_dc, pc_hair._features_rest,
         None, None, pc_hair._orient_conf, viewspace, viewpoint_camera.world_view_transform,
         viewpoint_camera.full_proj_transform, viewpoint_camera.camera_center, _tanfov_tensor(viewpoint_camera), st)
+    return _post(renders, radii, viewspace)
+
+
+def render_hair_strands(viewpoint_camera, pc, pc_hair, pipe, bg_color: torch.Tensor, scaling_modifier: float = 1.0):
+    """`render_hair` for a GaussianModelCurves (src/scene/gaussian_model_strands.py:31) rendered straight from its
+    polylines: same contract and returned dictionary as render_hair, but the strand Gaussians are built inside the
+    kernels from the trained segment vectors `pc_hair._dirs` (S,L,3) and `pc_hair.pts_origins` (S,1,3) -- midpoints,
+    |d|/2 scales and parallel-transport rotations, what initialize_gaussians_hair() (:435-454) rebuilds in PyTorch --
+    so the trainer drops its initialize_gaussians_hair() call.  Also read: `scale` (the strand thickness, a (1,) CUDA
+    tensor or a float), `_features_dc`, `_features_rest`, `_orient_conf` (S*L rows, strand-major), `active_sh_degree`.
+    Gradients land in `.grad` of `_dirs`, `_features_dc`, `_features_rest`, `_orient_conf`, of `viewspace_points`
+    and of trainable camera tensors; set_nan_flag() works as with render_hair.  `pc` supplies the frozen head block
+    like in render_hair (None or an empty block: hair only).
+
+    This does NOT refresh `pc_hair._pts`, `_xyz` or `_rotation`: a trainer that calls `capture()` (which saves them)
+    runs the model's own initialize_gaussians_hair() under torch.no_grad() first.  The strand model has no
+    gradient-arena layout: an installed arena (projection.set_gradient_arena) raises."""
+    if projection._GRAD_ARENA["storage"] is not None:
+        raise RuntimeError("render_hair_strands: the strand model has no gradient-arena layout; remove the arena first")
+    dirs = pc_hair._dirs
+    if dirs.ndim != 3 or dirs.shape[-1] != 3 or dirs.shape[1] < 1:
+        raise RuntimeError(f"render_hair_strands: _dirs must be (S, L, 3), got {tuple(dirs.shape)}")
+    S, L = int(dirs.shape[0]), int(dirs.shape[1])
+    dev = dirs.device
+    origins = pc_hair.pts_origins
+    if origins.numel() != S * 3:
+        raise RuntimeError(f"render_hair_strands: pts_origins must be (S, 1, 3) = ({S}, 1, 3), got {tuple(origins.shape)}")
+    for name in ("_features_dc", "_features_rest", "_orient_conf"):
+        t = getattr(pc_hair, name)
+        if t.shape[0] != S * L:
+            raise RuntimeError(f"render_hair_strands: {name} must have S*L = {S * L} rows (strand-major), got {t.shape[0]}")
+    scale = pc_hair.scale
+    if not isinstance(scale, torch.Tensor):
+        scale = torch.full((1,), float(scale), dtype=torch.float32, device=dev)
+    head = _head_block(pc) if pc is not None else None
+    n_head = 0 if head is None else int(head["xyz"].shape[0])
+    viewspace = empty_rows(n_head + S * L, (3,), torch.float32, dev).requires_grad_(True)
+    st = _static(viewpoint_camera, bg_color, scaling_modifier, pc_hair.active_sh_degree, getattr(pipe, "debug", False),
+                 projection.HAIR_STRANDS)
+    st["head"] = head if n_head > 0 else None
+    st["strands"] = {"origins": origins.detach(), "S": S, "L": L}
+    renders, radii = _FusedRender.apply(
+        None, scale.detach(), None, dirs, pc_hair._features_dc, pc_hair._features_rest, None, None, pc_hair._orient_conf,
+        viewspace, viewpoint_camera.world_view_transform, viewpoint_camera.full_proj_transform,
+        viewpoint_camera.camera_center, _tanfov_tensor(viewpoint_camera), st)
     return _post(renders, radii, viewspace)

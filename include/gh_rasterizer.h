@@ -252,7 +252,14 @@ int gh_allreduce_p2p(const unsigned long long* peer_bufs, const unsigned long lo
  * projmatrix (4,4, row-vector convention) and campos (3).
  * flags: bits 0-1 scale activation (0 identity, 1 exp), 2-3 opacity (0 identity, 1 sigmoid, 2 constant 1),
  *   4-5 label (0 identity, 1 sigmoid, 2 constant 1, 3 constant 0), 6-7 orientation confidence (0 identity, 1 exp,
- *   3 constant 0), 8-9 direction feature (0: s_max * R[argmax s], 1: normalize(dirs), 2: zero).
+ *   3 constant 0), 8-9 direction feature (0: s_max * R[argmax s], 1: normalize(dirs), 2: zero),
+ *   10 strand mode: Gaussian i is segment i of a polyline (src/scene/gaussian_model_strands.py:435-454) and its
+ *   geometry is derived from the segment vector d = dirs[i]: scales (|d|/2, scale, scale), rotation
+ *   parallel_transport(e_x, d).  `scaling` then points to ONE device float, the strand thickness `scale` (no host
+ *   read); `rotation`, `d_scaling` and `d_rotation` must be NULL; `dirs` and `d_dirs` are required; the scale
+ *   activation must be 0 and the direction feature 1.  The backward folds the scale and rotation gradients into
+ *   d_dirs (the direct term of each segment) and writes the gradient w.r.t. the segment midpoint to d_xyz: finish
+ *   with gh_strand_backward.
  * det_eps: added to the 2-D determinant before inversion (1e-12 GaussianModel, 1e-7 strand models).
  * Forward outputs: means2D (P,3) NDC, colors (P,10), opacities (P,1), conic (P,3), cov3D (P,6) or NULL,
  *   visible (P) uint8 = the caller's prefilter.  Culled Gaussians are NOT compacted away: their conic is 0, which the
@@ -306,6 +313,19 @@ int gh_project_backward(
     float* d_xyz, float* d_scaling, float* d_rotation, float* d_dirs, float* d_features_dc, float* d_features_rest,
     float* d_opacity, float* d_label, float* d_orient_conf, float* d_means2D, float* d_camera,
     unsigned int* nan_flag, void* workspace, gh_stream_t stream);
+
+/*
+ * Strand geometry (src/scene/gaussian_model_strands.py:435-454) for the strand mode of the projection (flag bit 10).
+ * S strands of L segments, strand-major rows; device float32, contiguous.
+ * gh_strand_midpoints: origins (S,1,3), dirs (S,L,3) segment vectors -> xyz (S*L,3) segment midpoints
+ *   0.5 (p_k + p_{k+1}), p_0 = origin, p_{k+1} = origin + sum_{j<=k} d_j (a warp scan per strand; any L >= 1).
+ *   `xyz` may be a row block of a larger buffer.
+ * gh_strand_backward: d_xyz (S*L,3) = dL/d midpoint, d_dirs (S*L,3) = the direct terms the projection backward wrote;
+ *   d_dirs is overwritten IN PLACE with dL/dd_k = direct_k + 0.5 d_xyz_k + sum_{j>k} d_xyz_j.  nan_flag (device uint,
+ *   or NULL): OR-ed with 1 when any total is NaN.
+ */
+int gh_strand_midpoints(int S, int L, const float* origins, const float* dirs, float* xyz, gh_stream_t stream);
+int gh_strand_backward(int S, int L, const float* d_xyz, float* d_dirs, unsigned int* nan_flag, gh_stream_t stream);
 
 /*
  * "Next" row (SURVEY.md 8f-3): adaptive density control -- the outcome of the reference's densify_and_prune

@@ -8,12 +8,13 @@ its C ABI (include/gh_rasterizer.h).  PyTorch is used for device memory and the 
 from __future__ import annotations
 
 import ctypes as C
-from typing import Optional, Tuple
+from typing import Tuple
 
 import torch
 
 from . import _capi
-from ._alloc import empty_rows, row_capacity
+from ._alloc import carve_segments, empty_rows, row_capacity, segments_floats
+from ._capi import _f32 as _prep, _ptr, _stream
 
 NUM_CHANNELS = 10  # reference cuda_rasterizer/config.h:15
 
@@ -26,52 +27,22 @@ NUM_CHANNELS = 10  # reference cuda_rasterizer/config.h:15
 # caller only has to all-reduce `flat[:P * GRAD_FLOATS_TRAINABLE_NATIVE]`.  means2D follows: its gradient
 # is only read for the densification statistics (per-view NORMS are accumulated, so it must not be
 # summed over ranks as a gradient; dist.allreduce_densification_stats reduces the statistics instead).
-_GRAD_LAYOUT = (("rotations", 4), ("colors", NUM_CHANNELS), ("opacity", 1), ("means3D", 3), ("scales", 3),
-                ("means2D", 3), ("conic", 4), ("cov3D", 6))
+# (segment padding: _alloc.segments_floats)
+_GRAD_LAYOUT = tuple((k, n, (n,)) for k, n in (("rotations", 4), ("colors", NUM_CHANNELS), ("opacity", 1), ("means3D", 3),
+                                                ("scales", 3), ("means2D", 3), ("conic", 4), ("cov3D", 6)))
 _N_TRAINABLE_SEGMENTS = 5
 GRAD_FLOATS_TRAINABLE_NATIVE = 4 + NUM_CHANNELS + 1 + 3 + 3
-GRAD_FLOATS_PER_GAUSSIAN = sum(n for _, n in _GRAD_LAYOUT)
-
-
-def _seg_floats(P: int, n: int) -> int:
-    """Every arena segment is padded to a multiple of 4 floats: segments stay 16-byte aligned for any P and
-    a 4-float-granular all-reduce of the trainable prefix never touches the means2D segment behind it."""
-    return (P * n + 3) // 4 * 4
+GRAD_FLOATS_PER_GAUSSIAN = sum(n for _, n, _ in _GRAD_LAYOUT)
 
 
 def arena_floats(P: int) -> int:
     """float32 elements of the gradient arena for P Gaussians (34 * P when P % 4 == 0)."""
-    return sum(_seg_floats(P, n) for _, n in _GRAD_LAYOUT)
+    return segments_floats(P, _GRAD_LAYOUT)
 
 
 def trainable_floats(P: int) -> int:
     """Length of the arena prefix the optimizer consumes in the native call shape (21 * P when P % 4 == 0)."""
-    return sum(_seg_floats(P, n) for _, n in _GRAD_LAYOUT[:_N_TRAINABLE_SEGMENTS])
-
-
-def _ptr(t: Optional[torch.Tensor]):
-    """Device pointer or NULL for an absent optional (empty tensor, reference __init__.py:210-222)."""
-    if t is None or t.numel() == 0:
-        return None
-    return C.c_void_p(t.data_ptr())
-
-
-def _prep(t: torch.Tensor, name: str, device: torch.device, align: int = 4) -> torch.Tensor:
-    """contiguous float32 on `device`, like `.contiguous().data<float>()` in the reference binding."""
-    if t.numel() == 0:
-        return t
-    if t.dtype != torch.float32:
-        raise RuntimeError(f"expected scalar type Float but found {t.dtype} for argument '{name}'")
-    if t.device != device:
-        raise RuntimeError(f"argument '{name}' is on {t.device}, expected {device}")
-    t = t.contiguous()
-    if t.data_ptr() % align:
-        t = t.clone()
-    return t
-
-
-def _stream(device: torch.device):
-    return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+    return segments_floats(P, _GRAD_LAYOUT[:_N_TRAINABLE_SEGMENTS])
 
 
 def rasterize_gaussians(
@@ -114,17 +85,8 @@ def rasterize_gaussians(
         background = _prep(background, "background", device)
         M = int(sh.size(1)) if sh.numel() != 0 else 0
 
-        geom_bytes, img_bytes, geom_cap = C.c_size_t(), C.c_size_t(), C.c_size_t()
-        _capi.check(lib.gh_forward_workspace_sizes(P, W, H, C.byref(geom_bytes), C.byref(img_bytes)))
-        # bucketed sizes for the per-Gaussian buffers (see _alloc.py): a model that grows a little keeps hitting the
-        # allocator's cached blocks
-        _capi.check(lib.gh_forward_workspace_sizes(row_capacity(P), W, H, C.byref(geom_cap), None))
-        geomBuffer = torch.empty(geom_cap.value, **byte_opts)[:geom_bytes.value]
-        imgBuffer = torch.empty(img_bytes.value, **byte_opts)
-        radii = empty_rows(P, (), torch.int32, device)
+        geomBuffer, imgBuffer, radii = alloc_forward_workspaces(P, W, H, device)
         out_color = torch.empty((NUM_CHANNELS, H, W), dtype=torch.float32, device=device)
-        stream = _stream(device)
-
         n_rendered, max_len = C.c_int(0), C.c_int(0)
         _capi.check(lib.gh_forward_preprocess(
             P, int(degree), M, W, H,
@@ -134,28 +96,25 @@ def rasterize_gaussians(
             _ptr(viewmatrix), _ptr(projmatrix), _ptr(campos),
             float(tan_fovx), float(tan_fovy), int(bool(prefiltered)),
             _ptr(radii), _ptr(geomBuffer), _ptr(imgBuffer),
-            C.byref(n_rendered), C.byref(max_len), int(bool(debug)), stream))
+            C.byref(n_rendered), C.byref(max_len), int(bool(debug)), _stream(device)))
         R = int(n_rendered.value)
-
-        bin_bytes = C.c_size_t()
-        _capi.check(lib.gh_binning_workspace_size(R, C.byref(bin_bytes)))
-        binningBuffer = torch.empty(bin_bytes.value, **byte_opts)
-        _capi.check(lib.gh_forward_render(
-            P, W, H, _ptr(background), _ptr(colors), _ptr(radii),
-            _ptr(geomBuffer), _ptr(binningBuffer), _ptr(imgBuffer),
-            R, int(max_len.value), _ptr(out_color), int(bool(debug)), stream))
+        binningBuffer = _render(background, colors, radii, geomBuffer, imgBuffer, R, int(max_len.value), out_color, debug)
     return R, out_color, radii, geomBuffer, binningBuffer, imgBuffer
 
 
 def alloc_forward_workspaces(P: int, W: int, H: int, device: torch.device):
-    """(geomBuffer, imgBuffer, radii) of a forward pass -- what rasterize_gaussians allocates before its first native
-    call; used by the fused projection (projection.project_forward_binned), which fills them itself."""
+    """(geomBuffer, imgBuffer, radii) of a forward pass, for the first phase to fill: gh_forward_preprocess
+    (rasterize_gaussians) or gh_project_forward_binned (projection.project_forward_binned)."""
     lib = _capi.load()
     byte_opts = dict(dtype=torch.uint8, device=device)
-    geom_bytes, img_bytes, geom_cap = C.c_size_t(), C.c_size_t(), C.c_size_t()
-    _capi.check(lib.gh_forward_workspace_sizes(P, W, H, C.byref(geom_bytes), C.byref(img_bytes)))
-    _capi.check(lib.gh_forward_workspace_sizes(row_capacity(P), W, H, C.byref(geom_cap), None))
-    geomBuffer = torch.empty(geom_cap.value, **byte_opts)[:geom_bytes.value]
+    # the geometry workspace is allocated for the bucketed row capacity (see _alloc.py), so that a model that grows a
+    # little keeps hitting the allocator's cached blocks; the view handed out has the size for P rows
+    geom_bytes, img_bytes = [], C.c_size_t()
+    for rows in (row_capacity(P), P):
+        n = C.c_size_t()
+        _capi.check(lib.gh_forward_workspace_sizes(rows, W, H, C.byref(n), C.byref(img_bytes)))
+        geom_bytes.append(n.value)
+    geomBuffer = torch.empty(geom_bytes[0], **byte_opts)[:geom_bytes[1]]
     imgBuffer = torch.empty(img_bytes.value, **byte_opts)
     radii = empty_rows(P, (), torch.int32, device)
     return geomBuffer, imgBuffer, radii
@@ -166,21 +125,28 @@ def forward_render(background: torch.Tensor, colors: torch.Tensor, radii: torch.
                    debug: bool = False):
     """Second phase of the forward (emit, sort, blend) on workspaces whose first phase already ran
     (gh_forward_preprocess or gh_project_forward_binned).  -> (out_color (C,H,W), binningBuffer)."""
+    device = colors.device
+    with torch.cuda.device(device):
+        out_color = torch.empty((NUM_CHANNELS, int(image_height), int(image_width)), dtype=torch.float32, device=device)
+        binningBuffer = _render(_prep(background, "background", device), _prep(colors, "colors", device, align=8), radii,
+                                geomBuffer, imgBuffer, num_rendered, max_tile_len, out_color, debug)
+    return out_color, binningBuffer
+
+
+def _render(background, colors, radii, geomBuffer, imgBuffer, num_rendered, max_tile_len, out_color, debug):
+    """gh_forward_render into `out_color` on prepared tensors, inside their device's context -> binningBuffer.
+    rasterize_gaussians calls this directly: between the first phase's read-back and this launch the GPU idles."""
     lib = _capi.load()
     device = colors.device
-    P, H, W = int(colors.shape[0]), int(image_height), int(image_width)
-    with torch.cuda.device(device):
-        background = _prep(background, "background", device)
-        colors = _prep(colors, "colors", device, align=8)
-        out_color = torch.empty((NUM_CHANNELS, H, W), dtype=torch.float32, device=device)
-        bin_bytes = C.c_size_t()
-        _capi.check(lib.gh_binning_workspace_size(int(num_rendered), C.byref(bin_bytes)))
-        binningBuffer = torch.empty(bin_bytes.value, dtype=torch.uint8, device=device)
-        _capi.check(lib.gh_forward_render(
-            P, W, H, _ptr(background), _ptr(colors), _ptr(radii),
-            _ptr(geomBuffer), _ptr(binningBuffer), _ptr(imgBuffer),
-            int(num_rendered), int(max_tile_len), _ptr(out_color), int(bool(debug)), _stream(device)))
-    return out_color, binningBuffer
+    H, W = int(out_color.size(1)), int(out_color.size(2))
+    bin_bytes = C.c_size_t()
+    _capi.check(lib.gh_binning_workspace_size(int(num_rendered), C.byref(bin_bytes)))
+    binningBuffer = torch.empty(bin_bytes.value, dtype=torch.uint8, device=device)
+    _capi.check(lib.gh_forward_render(
+        int(colors.shape[0]), W, H, _ptr(background), _ptr(colors), _ptr(radii),
+        _ptr(geomBuffer), _ptr(binningBuffer), _ptr(imgBuffer),
+        int(num_rendered), int(max_tile_len), _ptr(out_color), int(bool(debug)), _stream(device)))
+    return binningBuffer
 
 
 def alloc_grad_arena(P: int, device: torch.device, zero: bool = True, storage: torch.Tensor | None = None):
@@ -197,11 +163,33 @@ def alloc_grad_arena(P: int, device: torch.device, zero: bool = True, storage: t
     else:
         alloc = torch.zeros if zero else torch.empty
         flat = alloc(n, dtype=torch.float32, device=device)
-    views, off = {}, 0
-    for name, k in _GRAD_LAYOUT:
-        views[name] = flat[off:off + P * k].view(P, k)
-        off += _seg_floats(P, k)
-    return flat, views
+    return flat, carve_segments(flat, P, _GRAD_LAYOUT)
+
+
+def _backward(background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp, conic_precomp,
+              viewmatrix, projmatrix, tan_fovx, tan_fovy, dL_dout_color, sh, degree, campos, geomBuffer, R, binningBuffer,
+              imageBuffer, debug, grads=None, dL_dsh=None):
+    """gh_backward on prepared tensors (P > 0), arguments in the order of rasterize_gaussians_backward.  `grads`: the
+    alloc_grad_arena views that receive every per-Gaussian gradient; None leaves the blend's accumulation records in
+    `geomBuffer` (records mode, conic_precomp call shape)."""
+    device = means3D.device
+    P = int(means3D.size(0))
+    M = int(sh.size(1)) if sh is not None and sh.numel() != 0 else 0
+    H, W = int(dL_dout_color.size(1)), int(dL_dout_color.size(2))
+    g = grads or {}
+    with torch.cuda.device(device):
+        _capi.check(_capi.load().gh_backward(
+            P, int(degree), M, int(R), W, H,
+            _ptr(background), _ptr(means3D), _ptr(sh), _ptr(colors),
+            _ptr(scales), float(scale_modifier), _ptr(rotations),
+            _ptr(cov3D_precomp), _ptr(conic_precomp),
+            _ptr(viewmatrix), _ptr(projmatrix), _ptr(campos),
+            float(tan_fovx), float(tan_fovy), _ptr(radii),
+            _ptr(geomBuffer), _ptr(binningBuffer), _ptr(imageBuffer),
+            _ptr(dL_dout_color),
+            _ptr(g.get("means2D")), _ptr(g.get("conic")), _ptr(g.get("opacity")), _ptr(g.get("colors")),
+            _ptr(g.get("means3D")), _ptr(g.get("cov3D")), _ptr(dL_dsh), _ptr(g.get("scales")), _ptr(g.get("rotations")),
+            int(bool(debug)), _stream(device)))
 
 
 def rasterize_gaussians_backward_arena(
@@ -213,38 +201,19 @@ def rasterize_gaussians_backward_arena(
     per-Gaussian gradient is a (P, n) view into ONE flat float32 buffer, which is what a multi-GPU
     caller all-reduces (one collective per step, no packing copy).  `arena_storage` places the arena
     in caller-owned memory (a symmetric-memory buffer for dist.PeerAllReduce)."""
-    lib = _capi.load()
     device = means3D.device
     P = int(means3D.size(0))
-    H, W = int(dL_dout_color.size(1)), int(dL_dout_color.size(2))
     M = int(sh.size(1)) if sh.numel() != 0 else 0
     flat, g = alloc_grad_arena(P, device, zero=False, storage=arena_storage)     # gh_backward writes every element
     dL_dsh = torch.zeros((P, M, 3), dtype=torch.float32, device=device)
     if P != 0:
-        with torch.cuda.device(device):
-            means3D = _prep(means3D, "means3D", device)
-            colors = _prep(colors, "colors", device, align=8)
-            scales = _prep(scales, "scales", device)
-            rotations = _prep(rotations, "rotations", device, align=16)
-            cov3D_precomp = _prep(cov3D_precomp, "cov3D_precomp", device)
-            conic_precomp = _prep(conic_precomp, "conic_precomp", device)
-            viewmatrix = _prep(viewmatrix, "viewmatrix", device)
-            projmatrix = _prep(projmatrix, "projmatrix", device)
-            background = _prep(background, "background", device)
-            dL_dout_color = _prep(dL_dout_color, "dL_dout_color", device)
-            radii = radii.contiguous()
-            _capi.check(lib.gh_backward(
-                P, int(degree), M, int(R), W, H,
-                _ptr(background), _ptr(means3D), _ptr(sh), _ptr(colors),
-                _ptr(scales), float(scale_modifier), _ptr(rotations),
-                _ptr(cov3D_precomp), _ptr(conic_precomp),
-                _ptr(viewmatrix), _ptr(projmatrix), _ptr(campos),
-                float(tan_fovx), float(tan_fovy), _ptr(radii),
-                _ptr(geomBuffer), _ptr(binningBuffer), _ptr(imageBuffer),
-                _ptr(dL_dout_color),
-                _ptr(g["means2D"]), _ptr(g["conic"]), _ptr(g["opacity"]), _ptr(g["colors"]),
-                _ptr(g["means3D"]), _ptr(g["cov3D"]), _ptr(dL_dsh), _ptr(g["scales"]), _ptr(g["rotations"]),
-                int(bool(debug)), _stream(device)))
+        _backward(_prep(background, "background", device), _prep(means3D, "means3D", device), radii.contiguous(),
+                  _prep(colors, "colors", device, align=8), _prep(scales, "scales", device),
+                  _prep(rotations, "rotations", device, align=16), scale_modifier,
+                  _prep(cov3D_precomp, "cov3D_precomp", device), _prep(conic_precomp, "conic_precomp", device),
+                  _prep(viewmatrix, "viewmatrix", device), _prep(projmatrix, "projmatrix", device), tan_fovx, tan_fovy,
+                  _prep(dL_dout_color, "dL_dout_color", device), sh, degree, campos, geomBuffer, R, binningBuffer,
+                  imageBuffer, debug, g, dL_dsh)
     return flat, g, dL_dsh
 
 
@@ -254,26 +223,13 @@ def rasterize_gaussians_backward_records(background, means3D, radii, colors, con
     """Blend backward only, for the conic_precomp call shape: the per-Gaussian accumulation records (dL/d colour,
     2-D mean, conic, opacity) are LEFT in `geomBuffer` for `gh_project_backward` to consume directly -- no unpack
     pass, no intermediate gradient tensors (projection.project_backward(geom_buffer=...))."""
-    lib = _capi.load()
-    device = means3D.device
-    P = int(means3D.size(0))
-    if P == 0:
+    if int(means3D.size(0)) == 0:
         return
-    H, W = int(dL_dout_color.size(1)), int(dL_dout_color.size(2))
     if conic_precomp is None or conic_precomp.numel() == 0:
         raise RuntimeError("rasterize_gaussians_backward_records needs the conic_precomp call shape")
-    with torch.cuda.device(device):
-        dL = _prep(dL_dout_color, "dL_dout_color", device)
-        _capi.check(lib.gh_backward(
-            P, 0, 0, int(R), W, H,
-            _ptr(background), _ptr(means3D), None, _ptr(colors),
-            None, 1.0, None, None, _ptr(conic_precomp),
-            _ptr(viewmatrix), _ptr(projmatrix), _ptr(campos),
-            float(tan_fovx), float(tan_fovy), _ptr(radii),
-            _ptr(geomBuffer), _ptr(binningBuffer), _ptr(imageBuffer),
-            _ptr(dL),
-            None, None, None, None, None, None, None, None, None,
-            int(bool(debug)), _stream(device)))
+    _backward(background, means3D, radii, colors, None, None, 1.0, None, conic_precomp, viewmatrix, projmatrix,
+              tan_fovx, tan_fovy, _prep(dL_dout_color, "dL_dout_color", means3D.device), None, 0, campos,
+              geomBuffer, R, binningBuffer, imageBuffer, debug)
 
 
 def rasterize_gaussians_backward(

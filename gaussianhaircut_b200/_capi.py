@@ -1,13 +1,17 @@
 """ctypes binding of libgh_raster.so (C ABI: include/gh_rasterizer.h).
 
-Plain pointers and sizes only -- torch is used by the callers for device memory and streams, never
-here.  The library must have been built (python -m gaussianhaircut_b200.build); a missing library is
-a hard error, there is no fallback path.
+The library handle, the signature of every symbol, `check()` for its status codes, and the three helpers every
+caller uses to hand torch tensors to it: `_f32` (argument check), `_ptr` (device pointer or NULL) and `_stream`
+(the current CUDA stream).  Device memory is allocated by the callers.  The library must have been built
+(python -m gaussianhaircut_b200.build); a missing library is a hard error, there is no fallback path.
 """
 from __future__ import annotations
 
 import ctypes as C
 import os
+from typing import Optional
+
+import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libgh_raster.so")
@@ -25,6 +29,15 @@ _i = C.c_int
 _f = C.c_float
 _ll = C.c_longlong
 _sz = C.c_size_t
+
+# the leading arguments shared by gh_project_forward, gh_project_forward_binned and gh_project_backward
+_PROJ_ARGS = [
+    _i, _i, _i,                              # P width height
+    _p, _p, _p, _p,                          # xyz scaling rotation dirs
+    _p, _p,                                  # features_dc features_rest
+    _p, _p, _p,                              # opacity label orient_conf
+    _p, _p, _p,                              # viewmatrix projmatrix campos
+    _f, _f, _f, _i, C.c_uint, _f]            # tan_fovx tan_fovy scale_modifier sh_degree flags det_eps
 
 # name -> (restype, argtypes); every symbol declared in include/gh_rasterizer.h
 SIGNATURES = {
@@ -69,32 +82,14 @@ SIGNATURES = {
     "gh_allreduce_p2p": (_i, [_p, _p, C.c_ulonglong, _i, _i, C.c_size_t, C.c_size_t, C.c_uint, _p, _p, _p]),
     "gh_image_loss": (_i, [_i, _i, _p, _p, _p, _p, _p, _f, _f, _f, _f, _p, _p, _p, _p]),
     "gh_project_workspace_size": (_i, [_i, C.POINTER(C.c_size_t)]),
-    "gh_project_forward": (_i, [
-        _i, _i, _i,                          # P width height
-        _p, _p, _p, _p,                      # xyz scaling rotation dirs
-        _p, _p,                              # features_dc features_rest
-        _p, _p, _p,                          # opacity label orient_conf
-        _p, _p, _p,                          # viewmatrix projmatrix campos
-        _f, _f, _f, _i, C.c_uint, _f,        # tan_fovx tan_fovy scale_modifier sh_degree flags det_eps
+    "gh_project_forward": (_i, _PROJ_ARGS + [
         _p, _p, _p, _p, _p, _p,              # means2D colors opacities conic cov3D visible
         _p]),                                # stream
-    "gh_project_forward_binned": (_i, [
-        _i, _i, _i,
-        _p, _p, _p, _p,
-        _p, _p,
-        _p, _p, _p,
-        _p, _p, _p,
-        _f, _f, _f, _i, C.c_uint, _f,
+    "gh_project_forward_binned": (_i, _PROJ_ARGS + [
         _p, _p, _p, _p, _p, _p,              # means2D colors opacities conic cov3D visible
         _p, _p, _p, C.POINTER(C.c_int), C.POINTER(C.c_int),   # radii geom_buffer img_buffer num_rendered max_tile_len
         _p]),
-    "gh_project_backward": (_i, [
-        _i, _i, _i,
-        _p, _p, _p, _p,
-        _p, _p,
-        _p, _p, _p,
-        _p, _p, _p,
-        _f, _f, _f, _i, C.c_uint, _f,
+    "gh_project_backward": (_i, _PROJ_ARGS + [
         _p,                                  # visible
         _p,                                  # geom_buffer
         _p, _p, _p, _p,                      # dL_dmeans2D dL_dconic dL_dcolors dL_dopacity
@@ -157,3 +152,34 @@ def check(status: int) -> None:
     if status != GH_OK:
         msg = load().gh_last_error().decode("utf-8", "replace")
         raise GhError(status, msg or f"libgh_raster error {status}")
+
+
+def _ptr(t: Optional[torch.Tensor]):
+    """Device pointer of `t`, or NULL for an absent argument: None or an empty tensor (reference __init__.py:210-222)."""
+    if t is None or t.numel() == 0:
+        return None
+    return C.c_void_p(t.data_ptr())
+
+
+def _stream(device: torch.device):
+    return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+
+
+def _f32(t: Optional[torch.Tensor], name: str, device: torch.device, align: int = 4) -> Optional[torch.Tensor]:
+    """`t` as a detached contiguous float32 tensor on `device` whose data pointer is `align`-byte aligned (cloned if it
+    is not), like `.contiguous().data<float>()` in the reference binding.  An absent argument (None or an empty tensor,
+    on any device) is returned as it is."""
+    if t is None or t.numel() == 0:
+        return t
+    if not t.is_cuda:
+        raise RuntimeError(f"gaussianhaircut_b200: '{name}' must be a CUDA tensor (there is no CPU path)")
+    if t.dtype != torch.float32:
+        raise RuntimeError(f"expected scalar type Float but found {t.dtype} for argument '{name}'")
+    if t.device != device:
+        raise RuntimeError(f"argument '{name}' is on {t.device}, expected {device}")
+    if t.requires_grad:
+        t = t.detach()
+    t = t.contiguous()
+    if t.data_ptr() % align:
+        t = t.clone()
+    return t

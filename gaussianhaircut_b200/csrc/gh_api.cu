@@ -19,8 +19,6 @@ int gh_set_error(int code, const char* msg) {
 
 namespace {
 
-int gh_fail(int code, const char* msg) { return gh_set_error(code, msg); }
-
 int gh_check_cuda(cudaError_t e, const char* what) {
     if (e == cudaSuccess) return GH_OK;
     std::snprintf(g_err, sizeof(g_err), "[CUDA ERROR] %s: %s", what, cudaGetErrorString(e));
@@ -71,11 +69,6 @@ struct GhStageTimer {
     }
 };
 
-inline void gh_grid(int W, int H, int& gx, int& gy) {
-    gx = (W + GH_BLOCK_X - 1) / GH_BLOCK_X;
-    gy = (H + GH_BLOCK_Y - 1) / GH_BLOCK_Y;
-}
-
 __global__ void gh_export_keys_kernel(const uint2* __restrict__ ranges, const uint64_t* __restrict__ inst,
                                       unsigned long long* __restrict__ keys, unsigned int* __restrict__ plist)
 {
@@ -104,6 +97,38 @@ __global__ void gh_export_geom_kernel(int P, const GhGeo* __restrict__ geo, floa
 
 void gh_count_launches(int n) { g_launches.fetch_add((unsigned long long)n); }
 
+int gh_forward_phase1(const char* who, int P, int width, int height, char* geom_buffer, char* img_buffer, int* num_rendered,
+                      int* max_tile_len, int debug, cudaStream_t stream, GhBinLaunch launch, const void* bin)
+{
+    int gx, gy; const int T = gh_tile_grid(width, height, gx, gy);
+    if ((unsigned long long)gx * gx * gy >= (1ull << 32)) {    // exactness bound of the tile enumeration (gh_warp_rects)
+        std::snprintf(g_err, sizeof(g_err), "%s: image too large (tile grid gx * gx * gy must stay below 2^32)", who);
+        return GH_E_INVALID_ARG;
+    }
+    GhGeomWS geom = GhGeomWS::carve(geom_buffer, (size_t)P);
+    GhImgWS img = GhImgWS::carve(img_buffer, (size_t)width * height, (size_t)T);
+    // ctrl + tile histogram are contiguous: one memset
+    cudaError_t e = cudaMemsetAsync(img.ctrl, 0, 256 + gh_align_up((size_t)T * 4, 256), stream);
+    if (e != cudaSuccess) return gh_check_cuda(e, "memset(tile histogram)");
+    launch(bin, geom, img, gx, gy);
+    GH_STAGE(stream, debug, "preprocess");
+    {
+        GhStageTimer t(GH_ST_TILE_SCAN, stream);
+        gh_launch_tile_scan(T, img, stream);
+        g_launches += 1;
+    }
+    GH_STAGE(stream, debug, "tile scan");
+    GhCtrl h;
+    e = cudaMemcpyAsync(&h, img.ctrl, sizeof(GhCtrl), cudaMemcpyDeviceToHost, stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
+    if (e != cudaSuccess) return gh_check_cuda(e, "read back num_rendered");
+    *num_rendered = (int)h.num_rendered;
+    if (max_tile_len) *max_tile_len = (int)h.max_tile_len;
+    if (h.err_flags & GH_ERR_PREFILTERED)
+        return gh_set_error(GH_E_PREFILTERED, "Point is filtered although prefiltered is set. This shouldn't happen!");
+    return GH_OK;
+}
+
 extern "C" {
 
 int gh_abi_version(void) { return 3; }
@@ -127,8 +152,8 @@ const char* gh_last_error(void) { return g_err; }
 
 int gh_forward_workspace_sizes(int P, int width, int height, size_t* geom_bytes, size_t* img_bytes)
 {
-    if (P < 0 || width <= 0 || height <= 0) return gh_fail(GH_E_INVALID_ARG, "gh_forward_workspace_sizes: bad P/width/height");
-    int gx, gy; gh_grid(width, height, gx, gy);
+    if (P < 0 || width <= 0 || height <= 0) return gh_set_error(GH_E_INVALID_ARG, "gh_forward_workspace_sizes: bad P/width/height");
+    int gx, gy; gh_tile_grid(width, height, gx, gy);
     if (geom_bytes) *geom_bytes = GhGeomWS::bytes((size_t)P);
     if (img_bytes) *img_bytes = GhImgWS::bytes((size_t)width * height, (size_t)gx * gy);
     return GH_OK;
@@ -136,7 +161,7 @@ int gh_forward_workspace_sizes(int P, int width, int height, size_t* geom_bytes,
 
 int gh_binning_workspace_size(long long R, size_t* binning_bytes)
 {
-    if (R < 0) return gh_fail(GH_E_INVALID_ARG, "gh_binning_workspace_size: negative R");
+    if (R < 0) return gh_set_error(GH_E_INVALID_ARG, "gh_binning_workspace_size: negative R");
     if (binning_bytes) *binning_bytes = GhBinWS::bytes((size_t)R);
     return GH_OK;
 }
@@ -155,50 +180,23 @@ int gh_forward_preprocess(
     (void)D; (void)M; (void)means2D_precomp; (void)shs; (void)cam_pos;
     cudaStream_t stream = (cudaStream_t)stream_;
     g_err[0] = 0;
-    if (P <= 0 || width <= 0 || height <= 0) return gh_fail(GH_E_INVALID_ARG, "gh_forward_preprocess: P, width, height must be positive");
+    if (P <= 0 || width <= 0 || height <= 0) return gh_set_error(GH_E_INVALID_ARG, "gh_forward_preprocess: P, width, height must be positive");
     if (colors_precomp == nullptr)
-        return gh_fail(GH_E_NO_COLORS, "For non-RGB, provide precomputed Gaussian colors!");
+        return gh_set_error(GH_E_NO_COLORS, "For non-RGB, provide precomputed Gaussian colors!");
     if (!means3D || !opacities || !viewmatrix || !projmatrix || !radii || !geom_buffer || !img_buffer || !num_rendered)
-        return gh_fail(GH_E_INVALID_ARG, "gh_forward_preprocess: missing mandatory pointer");
+        return gh_set_error(GH_E_INVALID_ARG, "gh_forward_preprocess: missing mandatory pointer");
     if (conic_precomp == nullptr && cov3D_precomp == nullptr && (scales == nullptr || rotations == nullptr))
-        return gh_fail(GH_E_INVALID_ARG, "Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!");
-    if (rotations && ((size_t)rotations & 15)) return gh_fail(GH_E_INVALID_ARG, "rotations must be 16-byte aligned");
-    if (((size_t)colors_precomp & 7)) return gh_fail(GH_E_INVALID_ARG, "colors_precomp must be 8-byte aligned");
-
-    int gx, gy; gh_grid(width, height, gx, gy);
-    const int T = gx * gy;
-    if ((unsigned long long)gx * gx * gy >= (1ull << 32))     // exactness bound of the tile enumeration (gh_warp_rects)
-        return gh_fail(GH_E_INVALID_ARG, "gh_forward_preprocess: image too large (tile grid gx * gx * gy must stay below 2^32)");
-    GhGeomWS geom = GhGeomWS::carve(geom_buffer, (size_t)P);
-    GhImgWS img = GhImgWS::carve(img_buffer, (size_t)width * height, (size_t)T);
-
-    // ctrl + tile histogram are contiguous: one memset
-    cudaError_t e = cudaMemsetAsync(img.ctrl, 0, 256 + gh_align_up((size_t)T * 4, 256), stream);
-    if (e != cudaSuccess) return gh_check_cuda(e, "memset(tile histogram)");
-
-    {
+        return gh_set_error(GH_E_INVALID_ARG, "Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!");
+    if (rotations && ((size_t)rotations & 15)) return gh_set_error(GH_E_INVALID_ARG, "rotations must be 16-byte aligned");
+    if (((size_t)colors_precomp & 7)) return gh_set_error(GH_E_INVALID_ARG, "colors_precomp must be 8-byte aligned");
+    return gh_forward_phase1("gh_forward_preprocess", P, width, height, geom_buffer, img_buffer, num_rendered, max_tile_len,
+                             debug, stream, [&](const GhGeomWS& geom, const GhImgWS& img, int gx, int gy) {
         GhStageTimer t(GH_ST_PREPROCESS, stream);
         gh_launch_preprocess(P, means3D, scales, scale_modifier, rotations, opacities, cov3D_precomp,
                              conic_precomp, viewmatrix, projmatrix, width, height, tan_fovx, tan_fovy,
-                             radii, geom, img, prefiltered, stream);
+                             radii, geom, img, gx, gy, prefiltered, stream);
         g_launches += 1;
-    }
-    GH_STAGE(stream, debug, "preprocess");
-    {
-        GhStageTimer t(GH_ST_TILE_SCAN, stream);
-        gh_launch_tile_scan(T, img, stream);
-        g_launches += 1;
-    }
-    GH_STAGE(stream, debug, "tile scan");
-    GhCtrl h;
-    e = cudaMemcpyAsync(&h, img.ctrl, sizeof(GhCtrl), cudaMemcpyDeviceToHost, stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
-    if (e != cudaSuccess) return gh_check_cuda(e, "read back num_rendered");
-    *num_rendered = (int)h.num_rendered;
-    if (max_tile_len) *max_tile_len = (int)h.max_tile_len;
-    if (h.err_flags & GH_ERR_PREFILTERED)
-        return gh_fail(GH_E_PREFILTERED, "Point is filtered although prefiltered is set. This shouldn't happen!");
-    return GH_OK;
+    });
 }
 
 int gh_forward_render(
@@ -209,11 +207,10 @@ int gh_forward_render(
 {
     cudaStream_t stream = (cudaStream_t)stream_;
     g_err[0] = 0;
-    if (P <= 0 || width <= 0 || height <= 0 || num_rendered < 0) return gh_fail(GH_E_INVALID_ARG, "gh_forward_render: bad sizes");
+    if (P <= 0 || width <= 0 || height <= 0 || num_rendered < 0) return gh_set_error(GH_E_INVALID_ARG, "gh_forward_render: bad sizes");
     if (!background || !colors_precomp || !radii || !geom_buffer || !img_buffer || !out_color || (num_rendered > 0 && !binning_buffer))
-        return gh_fail(GH_E_INVALID_ARG, "gh_forward_render: missing mandatory pointer");
-    int gx, gy; gh_grid(width, height, gx, gy);
-    const int T = gx * gy;
+        return gh_set_error(GH_E_INVALID_ARG, "gh_forward_render: missing mandatory pointer");
+    int gx, gy; const int T = gh_tile_grid(width, height, gx, gy);
     GhGeomWS geom = GhGeomWS::carve(geom_buffer, (size_t)P);
     GhImgWS img = GhImgWS::carve(img_buffer, (size_t)width * height, (size_t)T);
     GhBinWS bin = GhBinWS::carve(binning_buffer, (size_t)num_rendered);
@@ -257,27 +254,26 @@ int gh_backward(
     (void)D; (void)M; (void)shs; (void)campos; (void)dL_dsh;
     cudaStream_t stream = (cudaStream_t)stream_;
     g_err[0] = 0;
-    if (P <= 0 || width <= 0 || height <= 0 || R < 0) return gh_fail(GH_E_INVALID_ARG, "gh_backward: bad sizes");
+    if (P <= 0 || width <= 0 || height <= 0 || R < 0) return gh_set_error(GH_E_INVALID_ARG, "gh_backward: bad sizes");
     // conic supplied + all four 2-D gradient outputs NULL: leave the accumulation records in the geometry workspace
     const bool keep_records = (conic_precomp != nullptr) && !dL_dmean2D && !dL_dconic && !dL_dopacity && !dL_dcolor;
     if (!background || !means3D || !colors_precomp || !viewmatrix || !projmatrix || !radii ||
         !geom_buffer || !img_buffer || !dL_dpix || (R > 0 && !binning_buffer) ||
         (!keep_records && (!dL_dmean2D || !dL_dconic || !dL_dopacity || !dL_dcolor)))
-        return gh_fail(GH_E_INVALID_ARG, "gh_backward: missing mandatory pointer");
+        return gh_set_error(GH_E_INVALID_ARG, "gh_backward: missing mandatory pointer");
     if (conic_precomp == nullptr) {
-        if (!dL_dmean3D || !dL_dcov3D) return gh_fail(GH_E_INVALID_ARG, "gh_backward: dL_dmean3D/dL_dcov3D required");
+        if (!dL_dmean3D || !dL_dcov3D) return gh_set_error(GH_E_INVALID_ARG, "gh_backward: dL_dmean3D/dL_dcov3D required");
         if (cov3D_precomp == nullptr && (!scales || !rotations || !dL_dscale || !dL_drot))
-            return gh_fail(GH_E_INVALID_ARG, "gh_backward: scales/rotations and their gradient buffers required");
-        if (rotations && ((size_t)rotations & 15)) return gh_fail(GH_E_INVALID_ARG, "rotations must be 16-byte aligned");
-        if (dL_drot && ((size_t)dL_drot & 15)) return gh_fail(GH_E_INVALID_ARG, "dL_drot must be 16-byte aligned");
+            return gh_set_error(GH_E_INVALID_ARG, "gh_backward: scales/rotations and their gradient buffers required");
+        if (rotations && ((size_t)rotations & 15)) return gh_set_error(GH_E_INVALID_ARG, "rotations must be 16-byte aligned");
+        if (dL_drot && ((size_t)dL_drot & 15)) return gh_set_error(GH_E_INVALID_ARG, "dL_drot must be 16-byte aligned");
     }
-    if (((size_t)colors_precomp & 7)) return gh_fail(GH_E_INVALID_ARG, "colors_precomp must be 8-byte aligned");
-    if (((size_t)dL_dconic & 15)) return gh_fail(GH_E_INVALID_ARG, "dL_dconic must be 16-byte aligned");
-    if (((size_t)dL_dcolor & 7)) return gh_fail(GH_E_INVALID_ARG, "dL_dcolor must be 8-byte aligned");
+    if (((size_t)colors_precomp & 7)) return gh_set_error(GH_E_INVALID_ARG, "colors_precomp must be 8-byte aligned");
+    if (((size_t)dL_dconic & 15)) return gh_set_error(GH_E_INVALID_ARG, "dL_dconic must be 16-byte aligned");
+    if (((size_t)dL_dcolor & 7)) return gh_set_error(GH_E_INVALID_ARG, "dL_dcolor must be 8-byte aligned");
     if (keep_records && (dL_dmean3D || dL_dcov3D || dL_dscale || dL_drot))
-        return gh_fail(GH_E_INVALID_ARG, "gh_backward: geometry gradients cannot be requested without the 2-D gradient outputs");
-    int gx, gy; gh_grid(width, height, gx, gy);
-    const int T = gx * gy;
+        return gh_set_error(GH_E_INVALID_ARG, "gh_backward: geometry gradients cannot be requested without the 2-D gradient outputs");
+    int gx, gy; const int T = gh_tile_grid(width, height, gx, gy);
     GhGeomWS geom = GhGeomWS::carve(geom_buffer, (size_t)P);
     GhImgWS img = GhImgWS::carve(img_buffer, (size_t)width * height, (size_t)T);
     GhBinWS bin = GhBinWS::carve(binning_buffer, (size_t)R);
@@ -327,9 +323,9 @@ int gh_mark_visible(int P, const float* means3D, const float* viewmatrix, const 
     (void)projmatrix;
     cudaStream_t stream = (cudaStream_t)stream_;
     g_err[0] = 0;
-    if (P < 0) return gh_fail(GH_E_INVALID_ARG, "gh_mark_visible: negative P");
+    if (P < 0) return gh_set_error(GH_E_INVALID_ARG, "gh_mark_visible: negative P");
     if (P == 0) return GH_OK;
-    if (!means3D || !viewmatrix || !present) return gh_fail(GH_E_INVALID_ARG, "gh_mark_visible: missing pointer");
+    if (!means3D || !viewmatrix || !present) return gh_set_error(GH_E_INVALID_ARG, "gh_mark_visible: missing pointer");
     gh_launch_mark_visible(P, means3D, viewmatrix, reinterpret_cast<bool*>(present), stream);
     GH_STAGE(stream, 0, "mark visible");
     return GH_OK;
@@ -345,9 +341,8 @@ int gh_debug_export(
     cudaStream_t stream = (cudaStream_t)stream_;
     g_err[0] = 0;
     if (P <= 0 || width <= 0 || height <= 0 || R < 0 || !geom_buffer || !img_buffer)
-        return gh_fail(GH_E_INVALID_ARG, "gh_debug_export: bad arguments");
-    int gx, gy; gh_grid(width, height, gx, gy);
-    const int T = gx * gy;
+        return gh_set_error(GH_E_INVALID_ARG, "gh_debug_export: bad arguments");
+    int gx, gy; const int T = gh_tile_grid(width, height, gx, gy);
     const size_t npix = (size_t)width * height;
     GhGeomWS geom = GhGeomWS::carve(const_cast<char*>(geom_buffer), (size_t)P);
     GhImgWS img = GhImgWS::carve(const_cast<char*>(img_buffer), npix, (size_t)T);

@@ -20,6 +20,13 @@
 #define GH_BLOCK_Y 16        // reference config.h:17
 #define GH_TILE_PIX (GH_BLOCK_X * GH_BLOCK_Y)
 
+// tiles of a width x height image: gx columns, gy rows; returns their number
+static inline int gh_tile_grid(int width, int height, int& gx, int& gy) {
+    gx = (width + GH_BLOCK_X - 1) / GH_BLOCK_X;
+    gy = (height + GH_BLOCK_Y - 1) / GH_BLOCK_Y;
+    return gx * gy;
+}
+
 // error bits in GhCtrl::err_flags
 #define GH_ERR_PREFILTERED 1u   // a point failed the near cull although prefiltered=true (auxiliary.h:156-160)
 

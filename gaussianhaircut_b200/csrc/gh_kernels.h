@@ -6,7 +6,7 @@ void gh_launch_preprocess(int P, const float* means3D, const float* scales, floa
                           const float* rotations, const float* opacities, const float* cov3D_precomp,
                           const float* conic_precomp, const float* viewmatrix, const float* projmatrix,
                           int W, int H, float tan_fovx, float tan_fovy, int* radii,
-                          GhGeomWS geom, GhImgWS img, int prefiltered, cudaStream_t stream);
+                          GhGeomWS geom, GhImgWS img, int gx, int gy, int prefiltered, cudaStream_t stream);
 
 void gh_launch_mark_visible(int P, const float* means3D, const float* viewmatrix, bool* present,
                             cudaStream_t stream);
@@ -46,6 +46,19 @@ void gh_launch_preprocess_backward(int P, const float* means3D, const int* radii
                                    float* dL_dopacity, float* dL_dcolor,
                                    float* dL_dmean3D, float* dL_dcov3D, float* dL_dscale, float* dL_drot,
                                    cudaStream_t stream);
+
+// The forward's first phase around its per-Gaussian kernel (gh_forward_preprocess, gh_project_forward_binned): tile grid
+// and its bound, workspace carving, ctrl + histogram memset, `bin(geom, img, gx, gy)` (launches the kernel on `stream` and
+// counts it), tile scan, read-back of R and the longest tile list.  `who` names the entry point in error messages.
+typedef void (*GhBinLaunch)(const void* bin, const GhGeomWS& geom, const GhImgWS& img, int gx, int gy);
+int gh_forward_phase1(const char* who, int P, int width, int height, char* geom_buffer, char* img_buffer, int* num_rendered,
+                      int* max_tile_len, int debug, cudaStream_t stream, GhBinLaunch launch, const void* bin);
+template <class F>
+int gh_forward_phase1(const char* who, int P, int width, int height, char* geom_buffer, char* img_buffer, int* num_rendered,
+                      int* max_tile_len, int debug, cudaStream_t stream, const F& bin) {
+    return gh_forward_phase1(who, P, width, height, geom_buffer, img_buffer, num_rendered, max_tile_len, debug, stream,
+                             [](const void* f, const GhGeomWS& g, const GhImgWS& i, int gx, int gy) { (*static_cast<const F*>(f))(g, i, gx, gy); }, &bin);
+}
 
 // per-thread error message behind gh_last_error(): every extern "C" entry point clears it on entry and
 // sets it before returning a GH_E_* code (defined in gh_api.cu)

@@ -143,9 +143,8 @@ void gh_launch_preprocess(int P, const float* means3D, const float* scales, floa
                           const float* rotations, const float* opacities, const float* cov3D_precomp,
                           const float* conic_precomp, const float* viewmatrix, const float* projmatrix,
                           int W, int H, float tan_fovx, float tan_fovy, int* radii,
-                          GhGeomWS geom, GhImgWS img, int prefiltered, cudaStream_t stream)
+                          GhGeomWS geom, GhImgWS img, int gx, int gy, int prefiltered, cudaStream_t stream)
 {
-    const int gx = (W + GH_BLOCK_X - 1) / GH_BLOCK_X, gy = (H + GH_BLOCK_Y - 1) / GH_BLOCK_Y;
     const float focal_y = H / (2.0f * tan_fovy);   // rasterizer_impl.cu:224-225
     const float focal_x = W / (2.0f * tan_fovx);
     gh_preprocess_kernel<<<(P + 127) / 128, 128, 0, stream>>>(

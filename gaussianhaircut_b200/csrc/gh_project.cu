@@ -345,9 +345,8 @@ extern "C" int gh_project_forward(
     return e == cudaSuccess ? GH_OK : gh_set_error(GH_E_CUDA, cudaGetErrorString(e));
 }
 
-// gh_project_forward + the rasterizer's first phase (gh_forward_preprocess) in one pass over the Gaussians: fills
-// radii and the geometry / image workspaces, runs the tile scan and reads back R like gh_forward_preprocess does;
-// continue with gh_forward_render.
+// gh_project_forward + the rasterizer's first phase (gh_forward_phase1, as in gh_forward_preprocess) in one pass over
+// the Gaussians; continue with gh_forward_render.
 extern "C" int gh_project_forward_binned(
     int P, int width, int height,
     const float* xyz, const float* scaling, const float* rotation, const float* dirs,
@@ -369,27 +368,13 @@ extern "C" int gh_project_forward_binned(
     if (!means2D || !colors || !opacities || !conic || !visible || !radii || !geom_buffer || !img_buffer || !num_rendered)
         return gh_set_error(GH_E_INVALID_ARG, "gh_project_forward_binned: missing output pointer");
     if ((size_t)colors & 7) return gh_set_error(GH_E_INVALID_ARG, "gh_project_forward_binned: colors must be 8-byte aligned");
-    const int gx = (width + GH_BLOCK_X - 1) / GH_BLOCK_X, gy = (height + GH_BLOCK_Y - 1) / GH_BLOCK_Y;
-    const int T = gx * gy;
-    if ((unsigned long long)gx * gx * gy >= (1ull << 32))     // exactness bound of the tile enumeration (gh_warp_rects)
-        return gh_set_error(GH_E_INVALID_ARG, "gh_project_forward_binned: image too large (tile grid gx * gx * gy must stay below 2^32)");
-    GhGeomWS geom = GhGeomWS::carve(geom_buffer, (size_t)P);
-    GhImgWS img = GhImgWS::carve(img_buffer, (size_t)width * height, (size_t)T);
-    // ctrl + tile histogram are contiguous: one memset
-    cudaError_t e = cudaMemsetAsync(img.ctrl, 0, 256 + gh_align_up((size_t)T * 4, 256), stream);
-    if (e != cudaSuccess) return gh_set_error(GH_E_CUDA, "gh_project_forward_binned: memset(tile histogram) failed");
     auto kernel = strand ? gh_project_forward_kernel<true, true> : gh_project_forward_kernel<true, false>;
-    kernel<<<(P + GH_PJ_THREADS - 1) / GH_PJ_THREADS, GH_PJ_THREADS, 0, stream>>>(
-        A, means2D, colors, opacities, conic, cov3D, visible, radii, geom.geo, geom.depth, img.tile_count, gx, gy);
-    gh_launch_tile_scan(T, img, stream);
-    gh_count_launches(2);
-    GhCtrl h;
-    e = cudaMemcpyAsync(&h, img.ctrl, sizeof(GhCtrl), cudaMemcpyDeviceToHost, stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
-    if (e != cudaSuccess) return gh_set_error(GH_E_CUDA, cudaGetErrorString(e));
-    *num_rendered = (int)h.num_rendered;
-    if (max_tile_len) *max_tile_len = (int)h.max_tile_len;
-    return GH_OK;
+    return gh_forward_phase1("gh_project_forward_binned", P, width, height, geom_buffer, img_buffer, num_rendered, max_tile_len,
+                             0, stream, [&](const GhGeomWS& geom, const GhImgWS& img, int gx, int gy) {
+        kernel<<<(P + GH_PJ_THREADS - 1) / GH_PJ_THREADS, GH_PJ_THREADS, 0, stream>>>(
+            A, means2D, colors, opacities, conic, cov3D, visible, radii, geom.geo, geom.depth, img.tile_count, gx, gy);
+        gh_count_launches(1);
+    });
 }
 
 extern "C" int gh_project_backward(

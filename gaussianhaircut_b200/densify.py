@@ -23,18 +23,11 @@ import torch
 from torch import nn
 
 from . import _capi
+from ._capi import _ptr, _stream
 
 # optimizer group name -> model attribute (src/scene/gaussian_model.py:431-442, :621-628)
 GROUPS = {"xyz": "_xyz", "f_dc": "_features_dc", "f_rest": "_features_rest", "opacity": "_opacity", "label": "_label",
           "scaling": "_scaling", "rotation": "_rotation", "orient_conf": "_orient_conf"}
-
-
-def _ptr(t: Optional[torch.Tensor]):
-    return None if t is None else C.c_void_p(t.data_ptr())
-
-
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
 
 
 def _pool_alloc(gaussians, key: str, rows: int, tail, dev, avoid: Optional[torch.Tensor]) -> torch.Tensor:

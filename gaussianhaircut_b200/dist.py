@@ -149,11 +149,10 @@ class PeerAllReduce:
             raise RuntimeError("PeerAllReduce: range must be 4-float aligned and inside the buffer")
         self._epoch += 1
         with torch.cuda.device(self.device):
-            stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
             self._capi.check(self._lib.gh_allreduce_p2p(
                 self._bufs, self._flagptrs, C.c_ulonglong(self.multicast), self.rank, self.world,
                 C.c_size_t(offset_floats), C.c_size_t(n), C.c_uint(self._epoch),
-                C.c_void_p(self._local.data_ptr()), C.c_void_p(self.nan_flag.data_ptr()), stream))
+                self._capi._ptr(self._local), self._capi._ptr(self.nan_flag), self._capi._stream(self.device)))
         if check and not self.ok():
             raise RuntimeError("PeerAllReduce: a peer did not reach the barrier in time; the reduction was skipped "
                                "and the gradient arena is undefined (GH_ALLREDUCE_TIMEOUT_MS)")

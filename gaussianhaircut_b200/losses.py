@@ -22,12 +22,9 @@ from typing import Dict, Tuple
 import torch
 
 from . import _capi
+from ._capi import _ptr, _stream
 
 __all__ = ["hair_image_loss", "HairImageLoss", "image_loss_forward_backward", "workspace_elems"]
-
-
-def _ptr(t: torch.Tensor):
-    return C.c_void_p(t.data_ptr())
 
 
 def _check(name: str, t: torch.Tensor, shape) -> torch.Tensor:
@@ -62,10 +59,9 @@ def image_loss_forward_backward(out: torch.Tensor, gt_image: torch.Tensor, gt_ma
     losses = torch.empty(8, dtype=torch.float32, device=dev)
     dL = torch.empty_like(out_c)
     with torch.cuda.device(dev):
-        stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
         _capi.check(lib.gh_image_loss(W, H, _ptr(out_c), _ptr(gi), _ptr(gm), _ptr(ga), _ptr(gc),
                                       float(l_dl1), float(l_dssim), float(l_dmask), float(l_dorient),
-                                      _ptr(workspace), _ptr(losses), _ptr(dL), stream))
+                                      _ptr(workspace), _ptr(losses), _ptr(dL), _stream(dev)))
     return losses, dL
 
 

@@ -21,6 +21,7 @@ from typing import Dict, Iterable, List, Optional, Sequence
 import torch
 
 from . import _capi
+from ._capi import _ptr, _stream
 
 MAX_GROUPS = 8   # GH_ADAM_MAX_GROUPS
 
@@ -131,10 +132,7 @@ class FusedAdam:
             _capi.check(lib.gh_adam_step(
                 n, arr(ps), arr(gs), arr(ms), arr(vs), (C.c_ulonglong * n)(*ns), (C.c_float * n)(*lrs),
                 float(self.betas[0]), float(self.betas[1]), float(self.eps), 0,
-                C.c_void_p(self.step_state.data_ptr()),
-                C.c_void_p(own_nan.data_ptr()) if own_nan is not None else None,
-                C.c_void_p(skip.data_ptr()) if skip is not None else None,
-                C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+                _ptr(self.step_state), _ptr(own_nan), _ptr(skip), _stream(dev)))
         if nan_flag_in is not None:
             nan_flag_in.zero_()       # consumed: ready for the next iteration's backward (stream-ordered after the update)
         self._keep = (ps, gs, skip)   # keep the tensors alive until the kernels have run

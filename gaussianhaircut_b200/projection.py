@@ -22,7 +22,8 @@ from typing import Dict, Optional
 import torch
 
 from . import _capi
-from ._alloc import empty_rows
+from ._alloc import carve_segments, empty_rows, segments_floats
+from ._capi import _f32, _ptr, _stream
 
 # activation / mode codes (GhProjArgs in csrc/gh_project_math.h)
 GAUSSIAN_MODEL = dict(scale_act=1, opacity_act=1, label_act=1, conf_act=1, dir_mode=0, det_eps=1e-12)   # gaussian_model.py
@@ -37,31 +38,6 @@ HAIR_STRANDS = dict(HAIR_MODEL, strands=1)
 def encode_flags(cfg: Dict[str, object]) -> int:
     return (int(cfg["scale_act"]) & 3) | ((int(cfg["opacity_act"]) & 3) << 2) | ((int(cfg["label_act"]) & 3) << 4) | \
            ((int(cfg["conf_act"]) & 3) << 6) | ((int(cfg["dir_mode"]) & 3) << 8) | ((int(cfg.get("strands", 0)) & 1) << 10)
-
-
-def _ptr(t: Optional[torch.Tensor]):
-    if t is None or t.numel() == 0:
-        return None
-    return C.c_void_p(t.data_ptr())
-
-
-def _f32(t: Optional[torch.Tensor], name: str, device: torch.device, align: int = 4) -> Optional[torch.Tensor]:
-    if t is None:
-        return None
-    if not t.is_cuda:
-        raise RuntimeError(f"gaussianhaircut_b200 projection: '{name}' must be a CUDA tensor (there is no CPU path)")
-    if t.dtype != torch.float32:
-        raise RuntimeError(f"expected scalar type Float but found {t.dtype} for argument '{name}'")
-    if t.device != device:
-        raise RuntimeError(f"argument '{name}' is on {t.device}, expected {device}")
-    t = t.detach().contiguous()
-    if t.data_ptr() % align:
-        t = t.clone()
-    return t
-
-
-def _stream(device):
-    return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
 
 class ProjectionInputs:
@@ -178,34 +154,37 @@ def _camera_workspace(P: int, dev: torch.device) -> torch.Tensor:
     return ws
 
 
-# parameter-gradient segments of a flat gradient arena (floats per Gaussian), in this order; every segment is padded to a
-# multiple of 4 floats so that a 4-float-granular all-reduce covers whole segments and every view stays 16-byte aligned
-GRAD_SEGMENTS = (("rotation", 4), ("xyz", 3), ("scaling", 3), ("f_dc", 3), ("f_rest", 45), ("opacity", 1), ("label", 1), ("conf", 1),
-                 ("dirs", 3))
+# the parameter gradients of project_backward, in the order of the flat gradient arena (segment padding:
+# _alloc.segments_floats); `dirs` is last and only there for models that have direction vectors
+GRAD_SEGMENTS = (("rotation", 4, (4,)), ("xyz", 3, (3,)), ("scaling", 3, (3,)), ("f_dc", 3, (1, 3)), ("f_rest", 45, (15, 3)),
+                 ("opacity", 1, (1,)), ("label", 1, (1,)), ("conf", 1, (1,)), ("dirs", 3, (3,)))
+
+
+def _grad_layout(with_dirs: bool):
+    return GRAD_SEGMENTS if with_dirs else GRAD_SEGMENTS[:-1]
 
 
 def grad_arena_floats(P: int, with_dirs: bool = False) -> int:
     """float32 elements of the model-gradient arena for P Gaussians (61 per Gaussian + padding; +3 with `dirs`)."""
-    return sum((P * n + 3) // 4 * 4 for k, n in GRAD_SEGMENTS if with_dirs or k != "dirs")
+    return segments_floats(P, _grad_layout(with_dirs))
 
 
 def carve_grad_arena(storage: torch.Tensor, P: int, with_dirs: bool = False) -> Dict[str, torch.Tensor]:
     need = grad_arena_floats(P, with_dirs)
     if storage.dtype != torch.float32 or not storage.is_contiguous() or storage.numel() < need:
         raise RuntimeError(f"projection: gradient arena must be a contiguous float32 tensor of at least {need} elements")
-    flat = storage.view(-1)
-    out, off = {}, 0
-    shapes = {"f_dc": (P, 1, 3), "f_rest": (P, 15, 3)}
-    for k, n in GRAD_SEGMENTS:
-        if k == "dirs" and not with_dirs:
-            continue
-        out[k] = flat[off:off + P * n].view(shapes.get(k, (P, n)))
-        off += (P * n + 3) // 4 * 4
-    return out
+    return carve_segments(storage.view(-1), P, _grad_layout(with_dirs))
 
 
 # process-wide, like rasterizer.set_gradient_arena (autograd's backward thread must see it)
-_GRAD_ARENA = {"storage": None, "last": None}
+_GRAD_ARENA = {"storage": None}
+
+
+def _check_no_strand_arena() -> None:
+    """The strand model has no gradient-arena layout: an installed arena raises (render_hair_strands checks before it
+    launches anything, project_backward again for direct callers)."""
+    if _GRAD_ARENA["storage"] is not None:
+        raise RuntimeError("projection: the strand model has no gradient-arena layout; remove the arena (set_gradient_arena(None))")
 
 
 def set_gradient_arena(storage):
@@ -214,7 +193,6 @@ def set_gradient_arena(storage):
     data-parallel trainer reduces the whole model gradient with ONE collective over `flat[:grad_arena_floats(P)]`."""
     prev = _GRAD_ARENA["storage"]
     _GRAD_ARENA["storage"] = storage
-    _GRAD_ARENA["last"] = None
     return prev
 
 
@@ -230,32 +208,23 @@ def project_backward(pi: ProjectionInputs, visible: torch.Tensor, geom_buffer: O
     dev, P = pi.device, pi.P
     f = dict(dtype=torch.float32, device=dev)
     strand = bool(pi.flags >> 10 & 1)
-    if strand and _GRAD_ARENA["storage"] is not None:
-        raise RuntimeError("projection: the strand model has no gradient-arena layout; remove the arena (set_gradient_arena(None))")
+    if strand:
+        _check_no_strand_arena()
+    # which gradients this model configuration has: the strand model folds scaling and rotation into dirs
+    has = {"scaling": not strand, "rotation": not strand, "dirs": pi.dirs is not None, "opacity": pi.opacity is not None,
+           "label": pi.label is not None, "conf": pi.conf is not None}
     if _GRAD_ARENA["storage"] is not None:
-        a = carve_grad_arena(_GRAD_ARENA["storage"], P, with_dirs=pi.dirs is not None)
-        _GRAD_ARENA["last"] = P
-        g = {"xyz": a["xyz"], "scaling": a["scaling"], "rotation": a["rotation"], "dirs": a.get("dirs"),
-             "f_dc": a["f_dc"], "f_rest": a["f_rest"],
-             "opacity": a["opacity"] if pi.opacity is not None else None,
-             "label": a["label"] if pi.label is not None else None,
-             "conf": a["conf"] if pi.conf is not None else None}
-        del a
+        views = carve_grad_arena(_GRAD_ARENA["storage"], P, with_dirs=has["dirs"])
     else:
-        f32 = torch.float32
-        g = {"xyz": empty_rows(P, (3,), f32, dev),
-             "scaling": None if strand else empty_rows(P, (3,), f32, dev), "rotation": None if strand else empty_rows(P, (4,), f32, dev),
-             "dirs": empty_rows(P, (3,), f32, dev) if pi.dirs is not None else None,
-             "f_dc": empty_rows(P, (1, 3), f32, dev), "f_rest": empty_rows(P, (15, 3), f32, dev),
-             "opacity": empty_rows(P, (1,), f32, dev) if pi.opacity is not None else None,
-             "label": empty_rows(P, (1,), f32, dev) if pi.label is not None else None,
-             "conf": empty_rows(P, (1,), f32, dev) if pi.conf is not None else None}
+        views = {k: empty_rows(P, shape, torch.float32, dev) for k, _, shape in GRAD_SEGMENTS if has.get(k, True)}
+    g = {k: views[k] if has.get(k, True) else None for k, _, _ in GRAD_SEGMENTS}
+    del views
     g["means2D"] = empty_rows(P, (3,), torch.float32, dev) if want_means2D_grad else None
     cam = torch.zeros(37, **f) if camera_grads else None
     if P != 0:
         with torch.cuda.device(dev):
             ws = _camera_workspace(P, dev) if camera_grads else None
-            conic4 = None if dL_dconic4 is None else _f32(dL_dconic4, "dL_dconic", dev, align=16)
+            conic4 = _f32(dL_dconic4, "dL_dconic", dev, align=16)
             _capi.check(lib.gh_project_backward(
                 *_common_args(pi), _ptr(visible), _ptr(geom_buffer),
                 _ptr(_f32(dL_dmeans2D, "dL_dmeans2D", dev)), _ptr(conic4), _ptr(_f32(dL_dcolors, "dL_dcolors", dev, align=8)),

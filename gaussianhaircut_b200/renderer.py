@@ -262,8 +262,7 @@ def render_hair_strands(viewpoint_camera, pc, pc_hair, pipe, bg_color: torch.Ten
     This does NOT refresh `pc_hair._pts`, `_xyz` or `_rotation`: a trainer that calls `capture()` (which saves them)
     runs the model's own initialize_gaussians_hair() under torch.no_grad() first.  The strand model has no
     gradient-arena layout: an installed arena (projection.set_gradient_arena) raises."""
-    if projection._GRAD_ARENA["storage"] is not None:
-        raise RuntimeError("render_hair_strands: the strand model has no gradient-arena layout; remove the arena first")
+    projection._check_no_strand_arena()
     dirs = pc_hair._dirs
     if dirs.ndim != 3 or dirs.shape[-1] != 3 or dirs.shape[1] < 1:
         raise RuntimeError(f"render_hair_strands: _dirs must be (S, L, 3), got {tuple(dirs.shape)}")

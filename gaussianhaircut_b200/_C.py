@@ -171,14 +171,23 @@ def _backward(background, means3D, radii, colors, scales, rotations, scale_modif
               imageBuffer, debug, grads=None, dL_dsh=None):
     """gh_backward on prepared tensors (P > 0), arguments in the order of rasterize_gaussians_backward.  `grads`: the
     alloc_grad_arena views that receive every per-Gaussian gradient; None leaves the blend's accumulation records in
-    `geomBuffer` (records mode, conic_precomp call shape)."""
+    `geomBuffer` (records mode, conic_precomp call shape).
+
+    Under `torch.use_deterministic_algorithms(True)` the deterministic blend backward runs (fixed summation order:
+    bit-reproducible gradients, slower); otherwise the fast path, whose float sums depend on GPU scheduling."""
     device = means3D.device
     P = int(means3D.size(0))
     M = int(sh.size(1)) if sh is not None and sh.numel() != 0 else 0
     H, W = int(dL_dout_color.size(1)), int(dL_dout_color.size(2))
     g = grads or {}
+    lib = _capi.load()
+    det_buffer, det_bytes = None, 0
+    if torch.are_deterministic_algorithms_enabled():
+        n = C.c_size_t()
+        _capi.check(lib.gh_backward_det_workspace_size(P, int(R), C.byref(n)))
+        det_buffer, det_bytes = torch.empty(n.value, dtype=torch.uint8, device=device), n.value
     with torch.cuda.device(device):
-        _capi.check(_capi.load().gh_backward(
+        _capi.check(lib.gh_backward(
             P, int(degree), M, int(R), W, H,
             _ptr(background), _ptr(means3D), _ptr(sh), _ptr(colors),
             _ptr(scales), float(scale_modifier), _ptr(rotations),
@@ -189,7 +198,7 @@ def _backward(background, means3D, radii, colors, scales, rotations, scale_modif
             _ptr(dL_dout_color),
             _ptr(g.get("means2D")), _ptr(g.get("conic")), _ptr(g.get("opacity")), _ptr(g.get("colors")),
             _ptr(g.get("means3D")), _ptr(g.get("cov3D")), _ptr(dL_dsh), _ptr(g.get("scales")), _ptr(g.get("rotations")),
-            int(bool(debug)), _stream(device)))
+            int(bool(debug)), _stream(device), _ptr(det_buffer), det_bytes))
 
 
 def rasterize_gaussians_backward_arena(

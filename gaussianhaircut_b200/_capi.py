@@ -22,7 +22,7 @@ GH_E_NO_COLORS = 2
 GH_E_CUDA = 3
 GH_E_PREFILTERED = 4
 
-ABI_VERSION = 3
+ABI_VERSION = 4
 
 _p = C.c_void_p
 _i = C.c_int
@@ -49,6 +49,7 @@ SIGNATURES = {
     "gh_stage_timing_read": (_i, [C.POINTER(C.c_double), C.POINTER(C.c_ulonglong), _i]),
     "gh_forward_workspace_sizes": (_i, [_i, _i, _i, C.POINTER(_sz), C.POINTER(_sz)]),
     "gh_binning_workspace_size": (_i, [_ll, C.POINTER(_sz)]),
+    "gh_backward_det_workspace_size": (_i, [_i, _ll, C.POINTER(_sz)]),
     "gh_forward_preprocess": (_i, [
         _i, _i, _i, _i, _i,                  # P D M width height
         _p, _p, _p, _p, _p,                  # means3D means2D_precomp shs colors_precomp opacities
@@ -75,12 +76,13 @@ SIGNATURES = {
         _p,                                  # dL_dpix
         _p, _p, _p, _p,                      # dL_dmean2D dL_dconic dL_dopacity dL_dcolor
         _p, _p, _p, _p, _p,                  # dL_dmean3D dL_dcov3D dL_dsh dL_dscale dL_drot
-        _i, _p]),                            # debug stream
+        _i, _p,                              # debug stream
+        _p, _sz]),                           # det_buffer det_bytes (NULL, 0: the fast path)
     "gh_mark_visible": (_i, [_i, _p, _p, _p, _p, _p]),
     "gh_adam_step": (_i, [_i, _p, _p, _p, _p, _p, _p, _f, _f, _f, _i, _p, _p, _p, _p]),
     "gh_image_loss_workspace_size": (_i, [_i, _i, C.POINTER(C.c_size_t)]),
     "gh_allreduce_p2p": (_i, [_p, _p, C.c_ulonglong, _i, _i, C.c_size_t, C.c_size_t, C.c_uint, _p, _p, _p]),
-    "gh_image_loss": (_i, [_i, _i, _p, _p, _p, _p, _p, _f, _f, _f, _f, _p, _p, _p, _p]),
+    "gh_image_loss": (_i, [_i, _i, _p, _p, _p, _p, _p, _f, _f, _f, _f, _p, _p, _p, _p, _i]),
     "gh_project_workspace_size": (_i, [_i, C.POINTER(C.c_size_t)]),
     "gh_project_forward": (_i, _PROJ_ARGS + [
         _p, _p, _p, _p, _p, _p,              # means2D colors opacities conic cov3D visible

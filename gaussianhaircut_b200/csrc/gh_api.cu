@@ -131,7 +131,7 @@ int gh_forward_phase1(const char* who, int P, int width, int height, char* geom_
 
 extern "C" {
 
-int gh_abi_version(void) { return 3; }
+int gh_abi_version(void) { return 4; }
 
 unsigned long long gh_kernel_launch_count(void) { return g_launches.load(); }
 
@@ -163,6 +163,13 @@ int gh_binning_workspace_size(long long R, size_t* binning_bytes)
 {
     if (R < 0) return gh_set_error(GH_E_INVALID_ARG, "gh_binning_workspace_size: negative R");
     if (binning_bytes) *binning_bytes = GhBinWS::bytes((size_t)R);
+    return GH_OK;
+}
+
+int gh_backward_det_workspace_size(int P, long long R, size_t* bytes)
+{
+    if (P < 0 || R < 0 || R > 0xffffffffll) return gh_set_error(GH_E_INVALID_ARG, "gh_backward_det_workspace_size: bad P/R");
+    if (bytes) *bytes = GhDetWS::bytes((size_t)P, (size_t)R);
     return GH_OK;
 }
 
@@ -249,12 +256,16 @@ int gh_backward(
     const float* dL_dpix,
     float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor,
     float* dL_dmean3D, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot,
-    int debug, gh_stream_t stream_)
+    int debug, gh_stream_t stream_, char* det_buffer, size_t det_bytes)
 {
     (void)D; (void)M; (void)shs; (void)campos; (void)dL_dsh;
     cudaStream_t stream = (cudaStream_t)stream_;
     g_err[0] = 0;
     if (P <= 0 || width <= 0 || height <= 0 || R < 0) return gh_set_error(GH_E_INVALID_ARG, "gh_backward: bad sizes");
+    if (det_buffer == nullptr && det_bytes != 0)
+        return gh_set_error(GH_E_INVALID_ARG, "gh_backward: det_bytes given without a det_buffer");
+    if (det_buffer != nullptr && det_bytes < GhDetWS::bytes((size_t)P, (size_t)R))
+        return gh_set_error(GH_E_INVALID_ARG, "gh_backward: det_buffer smaller than gh_backward_det_workspace_size");
     // conic supplied + all four 2-D gradient outputs NULL: leave the accumulation records in the geometry workspace
     const bool keep_records = (conic_precomp != nullptr) && !dL_dmean2D && !dL_dconic && !dL_dopacity && !dL_dcolor;
     if (!background || !means3D || !colors_precomp || !viewmatrix || !projmatrix || !radii ||
@@ -292,7 +303,28 @@ int gh_backward(
                 if (e != cudaSuccess) return gh_check_cuda(e, "memset(gradients)");
             }
     }
-    if (R > 0) {
+    if (R > 0 && det_buffer != nullptr) {
+        // deterministic path: offsets of the Gaussian-major rows, per-tile rows, fixed-order gather into acc16
+        GhStageTimer t(GH_ST_BLEND_BWD, stream);
+        GhDetWS det = GhDetWS::carve(det_buffer, (size_t)P, (size_t)R);
+        g_launches += gh_launch_det_offsets(P, gx, gy, radii, geom, det, stream);
+        if (debug) {
+            uint32_t total = 0;
+            cudaError_t e = cudaMemcpyAsync(&total, det.off + P, sizeof(total), cudaMemcpyDeviceToHost, stream);
+            if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
+            if (e != cudaSuccess) return gh_check_cuda(e, "read back the row count");
+            if (total != (uint32_t)R)
+                return gh_set_error(GH_E_INVALID_ARG, "gh_backward: the tile rectangles of radii do not add up to R");
+        }
+        gh_launch_blend_backward_det(width, height, gx, gy, radii, geom, img, bin, det, colors_precomp, background, dL_dpix, stream);
+        gh_launch_det_gather(P, geom, det, stream);
+        g_launches += 2;
+        if (conic_precomp != nullptr && !keep_records) {
+            gh_launch_unpack_grads(P, geom, dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolor,
+                                   dL_dmean3D, dL_dcov3D, dL_dscale, dL_drot, stream);
+            g_launches += 1;
+        }
+    } else if (R > 0) {
         GhStageTimer t(GH_ST_BLEND_BWD, stream);
         cudaError_t e = cudaMemsetAsync(geom.acc16, 0, (size_t)P * 64, stream);
         if (e != cudaSuccess) return gh_check_cuda(e, "memset(accumulation records)");

@@ -604,13 +604,37 @@ __device__ __forceinline__ bool gh_bwd_pair(GhBwdPair& p, const float4 g0, const
     return ok0 | ok1;
 }
 
+// ---- deterministic instantiation (DET = true): no atomics.  The tile's partial sum for each instance of its list
+// leaves as one 64-byte row at a Gaussian-major slot (GhDetWS); gh_det_gather_kernel sums the rows of each
+// Gaussian in a fixed order afterwards.
+struct GhDetArgs {
+    const int* radii;          // the radii emit used: with geo.x, geo.y they give the tile rectangle
+    const uint32_t* off;       // [P + 1] first row of each Gaussian
+    float4* rows;              // [R][4]
+    int gy;
+};
+
+// Row of instance (Gaussian id, tile (tx, ty)): off[id] + the tile's row-major rank inside the Gaussian's tile
+// rectangle, from the same gh_get_rect call on the same inputs as emit (gh_binning.cu)
+__device__ __forceinline__ float4* gh_det_row(const GhDetArgs& d, float mx, float my, uint32_t id, int tx, int ty, int gx) {
+    int minx, miny, maxx, maxy;
+    gh_get_rect(mx, my, d.radii[id], gx, d.gy, minx, miny, maxx, maxy);
+    const uint32_t k = (uint32_t)((ty - miny) * (maxx - minx) + (tx - minx));
+    return d.rows + 4 * ((size_t)d.off[id] + k);
+}
+
+// Per-warp partial records of one 32-record list word, [warp][record][quad], after the staging buffers
+constexpr size_t kBwdDetPartBytes = (size_t)(GH_BWD_THREADS / 32) * 32 * 4 * sizeof(float4);
+
+template <bool DET>
 __global__ void __launch_bounds__(GH_BWD_THREADS, GH_BWD_MIN_CTAS)
 gh_blend_backward_kernel(const uint2* __restrict__ ranges, const uint32_t* __restrict__ tile_perm, const uint64_t* __restrict__ inst,
                          const GhGeo* __restrict__ geo, const float* __restrict__ features,
                          int W, int H, int gx, const float* __restrict__ bg,
                          const float* __restrict__ final_T, const uint32_t* __restrict__ n_contrib,
                          const float* __restrict__ dL_dpix,
-                         float* __restrict__ acc16)   // [P][16]: colors 0..9, mean2D x,y, conic x,y,w, opacity
+                         float* __restrict__ acc16,   // [P][16]: colors 0..9, mean2D x,y, conic x,y,w, opacity
+                         GhDetArgs det)               // DET only
 {
     extern __shared__ __align__(16) unsigned char gh_bwd_smem[];
     GhStageB& st = *reinterpret_cast<GhStageB*>(gh_bwd_smem);
@@ -646,6 +670,16 @@ gh_blend_backward_kernel(const uint2* __restrict__ ranges, const uint32_t* __res
     for (int w = 0; w < GH_BWD_THREADS / 32; w++) tile_last = max(tile_last, s_warp_last[w]);
     const int n = (int)tile_last;             // nothing beyond is blended by any pixel of this tile
     const int nchunks = (n + GH_BWD_CHUNK - 1) / GH_BWD_CHUNK;
+    if constexpr (DET) {                      // instances past tile_last: zero rows
+        const int len = (int)(rg.y - rg.x);
+        for (int j = n + tid; j < len; j += GH_BWD_THREADS) {
+            const uint32_t id = (uint32_t)inst[(size_t)rg.x + j];
+            const float2 m = *reinterpret_cast<const float2*>(geo + id);
+            float4* row = gh_det_row(det, m.x, m.y, id, tx, ty, gx);
+            const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
+            row[0] = z; row[1] = z; row[2] = z; row[3] = z;
+        }
+    }
     if (nchunks == 0) return;
     // staging slots per thread; the last one may be partial when the window is not a multiple of 128
     constexpr int PER_THREAD = (GH_BWD_CHUNK + GH_BWD_THREADS - 1) / GH_BWD_THREADS;
@@ -683,7 +717,9 @@ gh_blend_backward_kernel(const uint2* __restrict__ ranges, const uint32_t* __res
     // b and 32 + b; every warp computes the same ranking for itself) and each warp takes 16 neighbours of that
     // ranking.  Any assignment gives the same gradients up to the order of the float atomics.
     int blk;
-    {
+    if constexpr (DET) {
+        blk = 16 * warp + lane / 2;           // natural order: a warp's 16 blocks are neighbours, their lists overlap
+    } else {
         const int nw = (n - (nchunks - 1) * GH_BWD_CHUNK + 31) >> 5;
         uint32_t len0 = 0, len1 = 0;
         for (int w = 0; w < nw; w++) {
@@ -772,6 +808,62 @@ gh_blend_backward_kernel(const uint2* __restrict__ ranges, const uint32_t* __res
                 gh_build_lists_b(st, cnt, word, lane, tx0, ty0, base, s_glast[lane], s_glast[32 + lane]);
             __syncthreads();
         }
+        if constexpr (DET) {
+            // Word by word, back to front: the warp walks the UNION of its 16 blocks' hit words, so at each step all
+            // blocks evaluate the same Gaussian (a block that does not list it runs with pos = UINT_MAX: exact zeros,
+            // state kept).  Its 16 components are summed over the block's 2 lanes, then over the 16 blocks by a fixed
+            // butterfly, and stored as the warp's partial; after a barrier the 4 warps are summed in warp order and
+            // the tile's partial leaves as one row per instance.  Every sum has a fixed order.
+            const bool walk = (uint32_t)base < wlast;
+            float4* wpart = reinterpret_cast<float4*>(gh_bwd_smem + sizeof(GhStageB));   // [warp][record][quad]
+            float4* mine_part = wpart + warp * 32 * 4;
+            for (int wi = ((cnt + 31) >> 5) - 1; wi >= 0; wi--) {
+#pragma unroll
+                for (int i = 0; i < 4; i++) mine_part[lane + 32 * i] = make_float4(0.f, 0.f, 0.f, 0.f);
+                const uint32_t mine = walk ? st.bits[blk][wi] : 0u;
+                uint32_t uni = __reduce_or_sync(0xffffffffu, mine);
+                __syncwarp();
+                while (uni != 0u) {
+                    const int bpos = 31 - __clz(uni);
+                    uni &= ~(1u << bpos);
+                    const int jj = wi * 32 + bpos;
+                    const float4 g0 = st.g0[jj], g1 = st.g1[jj];
+                    const uint32_t pos = ((mine >> bpos) & 1u) ? (uint32_t)(base + jj) : 0xffffffffu;
+                    float v[16];
+                    const bool contrib = gh_bwd_pair(pr, g0, g1, &st.feat[jj * GH_HALF_C], pxf, pos, nddelx_dx, nddely_dy, v);
+                    if (!__any_sync(0xffffffffu, contrib)) continue;     // the record stays zero
+                    float4 s0, s1;
+                    gh_group2_reduce16(v, lane, s0, s1);
+#pragma unroll
+                    for (int o = 2; o < 32; o <<= 1) {
+                        s0.x += __shfl_xor_sync(0xffffffffu, s0.x, o); s0.y += __shfl_xor_sync(0xffffffffu, s0.y, o);
+                        s0.z += __shfl_xor_sync(0xffffffffu, s0.z, o); s0.w += __shfl_xor_sync(0xffffffffu, s0.w, o);
+                        s1.x += __shfl_xor_sync(0xffffffffu, s1.x, o); s1.y += __shfl_xor_sync(0xffffffffu, s1.y, o);
+                        s1.z += __shfl_xor_sync(0xffffffffu, s1.z, o); s1.w += __shfl_xor_sync(0xffffffffu, s1.w, o);
+                    }
+                    if (lane < 2) {                  // components 0..3, 8..11 (lane 0) / 4..7, 12..15 (lane 1)
+                        mine_part[bpos * 4 + lane] = s0;
+                        mine_part[bpos * 4 + 2 + lane] = s1;
+                    }
+                }
+                __syncthreads();
+                {
+                    const int r = tid >> 2, q = tid & 3, jj = wi * 32 + r;
+                    if (jj < cnt) {
+                        float4 a = wpart[r * 4 + q];
+#pragma unroll
+                        for (int w = 1; w < GH_BWD_THREADS / 32; w++) {
+                            const float4 b = wpart[(w * 32 + r) * 4 + q];
+                            a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
+                        }
+                        const float4 g0 = st.g0[jj];
+                        gh_det_row(det, g0.x, g0.y, st.id[jj], tx, ty, gx)[q] = a;
+                    }
+                }
+                __syncthreads();
+            }
+            continue;
+        }
         if ((uint32_t)base >= wlast) continue;
 
         int wi = (cnt + 31) >> 5;
@@ -837,6 +929,102 @@ gh_unpack_grads_kernel(int P, const float* __restrict__ acc16, float* __restrict
     if (dL_drot) reinterpret_cast<float4*>(dL_drot)[idx] = make_float4(0.f, 0.f, 0.f, 0.f);
 }
 
+// ---------------------------------------------------------------------------- deterministic backward: rows
+// Offsets of the Gaussian-major rows: off = exclusive prefix sum of the tile-rectangle areas (emit's rectangles:
+// 0 for radius <= 0), in three launches -- per-CTA sums, one CTA scanning those, per-CTA scans plus their offset.
+__device__ __forceinline__ uint32_t gh_det_area(int i, int P, const GhGeo* __restrict__ geo, const int* __restrict__ radii,
+                                                int gx, int gy) {
+    if (i >= P) return 0u;
+    const int r = radii[i];
+    if (r <= 0) return 0u;
+    const float2 m = *reinterpret_cast<const float2*>(geo + i);
+    int minx, miny, maxx, maxy;
+    gh_get_rect(m.x, m.y, r, gx, gy, minx, miny, maxx, maxy);
+    return (uint32_t)((maxx - minx) * (maxy - miny));
+}
+
+// exclusive scan of one value per thread over a 256-thread CTA; returns the CTA total through `total`
+__device__ __forceinline__ uint32_t gh_cta_scan256(uint32_t v, uint32_t* s_warp, uint32_t& total) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    uint32_t x = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const uint32_t nb = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += nb; }
+    if (lane == 31) s_warp[warp] = x;
+    __syncthreads();
+    uint32_t before = 0;
+    total = 0;
+#pragma unroll
+    for (int w = 0; w < 8; w++) { const uint32_t s = s_warp[w]; before += (w < warp) ? s : 0u; total += s; }
+    __syncthreads();
+    return before + x - v;
+}
+
+__global__ void __launch_bounds__(256)
+gh_det_area_sums_kernel(int P, const GhGeo* __restrict__ geo, const int* __restrict__ radii, int gx, int gy,
+                        uint32_t* __restrict__ part)
+{
+    __shared__ uint32_t s_warp[8];
+    const int i0 = blockIdx.x * GH_DET_SCAN_ITEMS + threadIdx.x * 4;
+    uint32_t s = 0;
+#pragma unroll
+    for (int k = 0; k < 4; k++) s += gh_det_area(i0 + k, P, geo, radii, gx, gy);
+    uint32_t total;
+    gh_cta_scan256(s, s_warp, total);
+    if (threadIdx.x == 0) part[blockIdx.x] = total;
+}
+
+__global__ void __launch_bounds__(256)
+gh_det_part_scan_kernel(int nb, int P, uint32_t* __restrict__ part, uint32_t* __restrict__ off)
+{
+    __shared__ uint32_t s_warp[8];
+    uint32_t carry = 0;
+    for (int b0 = 0; b0 < nb; b0 += 256) {
+        const int b = b0 + (int)threadIdx.x;
+        const uint32_t v = (b < nb) ? part[b] : 0u;
+        uint32_t total;
+        const uint32_t ex = gh_cta_scan256(v, s_warp, total);
+        if (b < nb) part[b] = carry + ex;
+        carry += total;
+    }
+    if (threadIdx.x == 0) off[P] = carry;       // = R
+}
+
+__global__ void __launch_bounds__(256)
+gh_det_offsets_kernel(int P, const GhGeo* __restrict__ geo, const int* __restrict__ radii, int gx, int gy,
+                      const uint32_t* __restrict__ part, uint32_t* __restrict__ off)
+{
+    __shared__ uint32_t s_warp[8];
+    const int i0 = blockIdx.x * GH_DET_SCAN_ITEMS + threadIdx.x * 4;
+    uint32_t a[4], s = 0;
+#pragma unroll
+    for (int k = 0; k < 4; k++) { a[k] = gh_det_area(i0 + k, P, geo, radii, gx, gy); s += a[k]; }
+    uint32_t total;
+    uint32_t run = part[blockIdx.x] + gh_cta_scan256(s, s_warp, total);
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+        if (i0 + k < P) off[i0 + k] = run;
+        run += a[k];
+    }
+}
+
+// acc16[i] = sum of rows off[i] .. off[i+1] in row order (4 threads per Gaussian, one float4 quad each); assigns every
+// record, so no clearing pass is needed
+__global__ void __launch_bounds__(256)
+gh_det_gather_kernel(int P, const uint32_t* __restrict__ off, const float4* __restrict__ rows, float4* __restrict__ acc16)
+{
+    const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const size_t i = t >> 2;
+    const int q = (int)(t & 3);
+    if (i >= (size_t)P) return;
+    const uint32_t r0 = off[i], r1 = off[i + 1];
+    float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (uint32_t r = r0; r < r1; r++) {
+        const float4 b = rows[4 * (size_t)r + q];
+        a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
+    }
+    acc16[4 * i + q] = a;
+}
+
 }  // namespace
 
 void gh_launch_blend_forward(int W, int H, int gx, int gy, GhGeomWS geom, GhImgWS img, GhBinWS bin,
@@ -857,11 +1045,40 @@ void gh_launch_blend_backward(int W, int H, int gx, int gy, GhGeomWS geom, GhImg
                               cudaStream_t stream)
 {
     const int smem = (int)sizeof(GhStageB);
-    cudaFuncSetAttribute(gh_blend_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    cudaFuncSetAttribute(gh_blend_backward_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
-    gh_blend_backward_kernel<<<gx * gy, GH_BWD_THREADS, smem, stream>>>(img.ranges, img.tile_perm, bin.inst, geom.geo, features,
+    cudaFuncSetAttribute(gh_blend_backward_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaFuncSetAttribute(gh_blend_backward_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    gh_blend_backward_kernel<false><<<gx * gy, GH_BWD_THREADS, smem, stream>>>(img.ranges, img.tile_perm, bin.inst, geom.geo, features,
                                                           W, H, gx, bg, img.final_T, img.n_contrib, dL_dpix,
-                                                          geom.acc16);
+                                                          geom.acc16, GhDetArgs{});
+}
+
+int gh_launch_det_offsets(int P, int gx, int gy, const int* radii, GhGeomWS geom, GhDetWS det, cudaStream_t stream)
+{
+    const int nb = (int)GhDetWS::scan_blocks((size_t)P);
+    gh_det_area_sums_kernel<<<nb, 256, 0, stream>>>(P, geom.geo, radii, gx, gy, det.part);
+    gh_det_part_scan_kernel<<<1, 256, 0, stream>>>(nb, P, det.part, det.off);
+    gh_det_offsets_kernel<<<nb, 256, 0, stream>>>(P, geom.geo, radii, gx, gy, det.part, det.off);
+    return 3;
+}
+
+void gh_launch_blend_backward_det(int W, int H, int gx, int gy, const int* radii, GhGeomWS geom, GhImgWS img, GhBinWS bin,
+                                  GhDetWS det, const float* features, const float* bg, const float* dL_dpix,
+                                  cudaStream_t stream)
+{
+    const int smem = (int)(sizeof(GhStageB) + kBwdDetPartBytes);
+    cudaFuncSetAttribute(gh_blend_backward_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaFuncSetAttribute(gh_blend_backward_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    const GhDetArgs d{radii, det.off, reinterpret_cast<float4*>(det.rows), gy};
+    gh_blend_backward_kernel<true><<<gx * gy, GH_BWD_THREADS, smem, stream>>>(img.ranges, img.tile_perm, bin.inst, geom.geo, features,
+                                                         W, H, gx, bg, img.final_T, img.n_contrib, dL_dpix,
+                                                         nullptr, d);
+}
+
+void gh_launch_det_gather(int P, GhGeomWS geom, GhDetWS det, cudaStream_t stream)
+{
+    const long long threads = 4ll * P;
+    gh_det_gather_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, stream>>>(
+        P, det.off, reinterpret_cast<const float4*>(det.rows), reinterpret_cast<float4*>(geom.acc16));
 }
 
 void gh_launch_unpack_grads(int P, GhGeomWS geom, float* dL_dmean2D, float* dL_dconic, float* dL_dopacity,

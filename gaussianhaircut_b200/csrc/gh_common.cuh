@@ -123,6 +123,28 @@ struct GhBinWS {
     }
 };
 
+// Workspace of the deterministic blend backward (gh_blend.cu): one 64-byte partial record per (Gaussian, tile)
+// instance, Gaussian-major -- the rows of Gaussian i are off[i] .. off[i+1], in row-major order of the tiles of its
+// rectangle -- the exclusive prefix sum `off` of the rectangle areas (off[P] = R), and the per-CTA sums of that scan.
+#define GH_DET_SCAN_ITEMS 1024   // Gaussians per CTA of the offset scan (256 threads x 4)
+struct GhDetWS {
+    float* rows;         // [R][16]
+    uint32_t* off;       // [P + 1]
+    uint32_t* part;      // [scan_blocks(P)]
+    static __host__ __device__ size_t scan_blocks(size_t P) { return (P + GH_DET_SCAN_ITEMS - 1) / GH_DET_SCAN_ITEMS; }
+    static __host__ __device__ size_t bytes(size_t P, size_t R) {
+        return gh_align_up(R * 64, 256) + gh_align_up((P + 1) * 4, 256) + gh_align_up(scan_blocks(P) * 4, 256) + 256;
+    }
+    static __host__ __device__ GhDetWS carve(char* base, size_t P, size_t R) {
+        GhDetWS w;
+        size_t off = gh_align_up((size_t)base, 256) - (size_t)base;
+        w.rows = (float*)(base + off); off += gh_align_up(R * 64, 256);
+        w.off = (uint32_t*)(base + off); off += gh_align_up((P + 1) * 4, 256);
+        w.part = (uint32_t*)(base + off);
+        return w;
+    }
+};
+
 #ifdef __CUDACC__
 // Tile rectangle of a splat (reference auxiliary.h:46-56, float->int truncation, clamp to grid).
 // PTX of the reference: (p - r) * 0.0625 ; ((p + r) + 16) + (-1)) * 0.0625 ; cvt.rzi ; max.s32 0 ; min.u32 grid

@@ -39,8 +39,7 @@ struct GhLossParams {
     float g[11];                       // normalised 1-D Gaussian window, sigma 1.5 (loss_utils.py:74-76)
 };
 
-// sums[]: 0 sum w, 1 sum |I-G| m, 2 sum ssim_map, 3 sum |M-GM|, 4 sum orient loss * w
-enum { GH_LS_W = 0, GH_LS_L1 = 1, GH_LS_SSIM = 2, GH_LS_MASK = 3, GH_LS_ORIENT = 4, GH_LS_COUNT = 8 };
+enum { GH_LS_W = 0, GH_LS_L1 = 1, GH_LS_SSIM = 2, GH_LS_MASK = 3, GH_LS_ORIENT = 4, GH_LS_COUNT = 16 };
 
 __device__ __forceinline__ float gh_sign(float x) { return (x > 0.f) ? 1.f : ((x < 0.f) ? -1.f : 0.f); }
 __device__ __forceinline__ float2 gh_l2(float a) { return make_float2(a, a); }
@@ -63,13 +62,93 @@ __device__ __forceinline__ void gh_block_add(double v, double* dst, double* s_pa
     }
 }
 
+// sums[] (doubles): 0 sum w, 1 sum |I-G| m, 2 sum ssim_map, 3 sum |M-GM|, 4 sum orient loss * w; slots 8.. hold the
+// completion tickets of the three summing kernels (uint32, zeroed with the sums)
+enum { GH_TK_PRESUM = 8, GH_TK_POINTWISE = 9, GH_TK_MAIN = 10 };
+
+// Deterministic variant of gh_block_add for K sums (gh_image_loss with deterministic != 0): warp shuffle tree, the 8
+// warps in warp order, then the CTA's total goes to its own slot part[k * gridDim + CTA] -- no floating-point atomics.
+// The last CTA to finish (ticket) adds the slots in CTA order into sums[idx[k]], staging 256 slots at a time in shared
+// memory; that is one of the orders the per-CTA atomicAdd could produce, now the only one, so the loss values and the
+// 1 / sum(w) that scales the orientation gradient are reproducible.
+template <int K>
+__device__ __forceinline__ void gh_block_sum_fixed(double (&v)[K], double* __restrict__ part, double* sums,
+                                                   const int (&idx)[K], int ticket_slot) {
+    __shared__ double s_part[K][8];
+    __shared__ bool s_last;
+    const int tid = threadIdx.x;
+#pragma unroll
+    for (int k = 0; k < K; k++) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], o);
+    }
+    __syncthreads();
+    if ((tid & 31) == 0) {
+#pragma unroll
+        for (int k = 0; k < K; k++) s_part[k][tid >> 5] = v[k];
+    }
+    __syncthreads();
+    const unsigned G = gridDim.x * gridDim.y, b = blockIdx.y * gridDim.x + blockIdx.x;
+    if (tid == 0) {
+#pragma unroll
+        for (int k = 0; k < K; k++) {
+            double t = 0.0;
+            for (int w = 0; w < 8; w++) t += s_part[k][w];
+            part[(size_t)k * G + b] = t;
+        }
+        __threadfence();
+        s_last = atomicAdd(reinterpret_cast<unsigned*>(sums + ticket_slot), 1u) == G - 1u;
+    }
+    __syncthreads();
+    if (!s_last) return;
+    __threadfence();
+    __shared__ double s_stage[K][256];
+    double t = 0.0;                     // thread k: sum k
+    for (unsigned c0 = 0; c0 < G; c0 += 256) {
+        const unsigned m = min(256u, G - c0);
+#pragma unroll
+        for (int k = 0; k < K; k++)
+            if ((unsigned)tid < m) s_stage[k][tid] = __ldcg(part + (size_t)k * G + c0 + tid);
+        __syncthreads();
+        if (tid < K)
+            for (unsigned i = 0; i < m; i++) t += s_stage[tid][i];
+        __syncthreads();
+    }
+    if (tid < K) {
+        int d = idx[0];
+#pragma unroll
+        for (int k = 1; k < K; k++) d = (tid == k) ? idx[k] : d;
+        sums[d] = t;
+    }
+}
+
+// per-CTA slots of the three summing kernels, after the sums: presum, pointwise (3 sums), SSIM
+struct GhLossParts {
+    int rb, pb, mb;                    // CTAs of presum / finalize, pointwise, main
+    static GhLossParts of(int W, int H) {
+        const size_t plane = (size_t)W * H;
+        GhLossParts p;
+        p.rb = (int)((plane + 255) / 256 < 132u * 8u ? (plane + 255) / 256 : 132u * 8u);
+        p.pb = (int)((plane + 255) / 256 < 132u * 16u ? (plane + 255) / 256 : 132u * 16u);
+        p.mb = ((W + GH_LT - 1) / GH_LT) * ((H + GH_LT - 1) / GH_LT);
+        return p;
+    }
+    size_t doubles() const { return (size_t)rb + 3 * (size_t)pb + (size_t)mb; }
+};
+
+template <bool DET>
 __global__ void __launch_bounds__(256)
-gh_loss_presum_kernel(const float* __restrict__ gt_orient_conf, size_t n, double* __restrict__ sums)
+gh_loss_presum_kernel(const float* __restrict__ gt_orient_conf, size_t n, double* __restrict__ sums, double* __restrict__ part)
 {
-    __shared__ double s_part[8];
     double acc = 0.0;
     for (size_t i = (size_t)blockIdx.x * 256 + threadIdx.x; i < n; i += (size_t)gridDim.x * 256) acc += (double)gt_orient_conf[i];
-    gh_block_add(acc, sums + GH_LS_W, s_part);
+    if constexpr (DET) {
+        double v[1] = {acc};
+        gh_block_sum_fixed<1>(v, part, sums, {GH_LS_W}, GH_TK_PRESUM);
+    } else {
+        __shared__ double s_part[8];
+        gh_block_add(acc, sums + GH_LS_W, s_part);
+    }
 }
 
 // Pointwise terms of one pixel: loss contributions (returned through the accumulators) and dL/dout for
@@ -138,35 +217,42 @@ __device__ __forceinline__ void gh_loss_pointwise(const GhLossParams& prm, size_
 
 // All pointwise terms (masked L1 value, mask L1, orientation) of every pixel: loss sums and dL/dout
 // channels 3..9.  Plain elementwise kernel, one pixel per thread per grid-stride step.
+template <bool DET>
 __global__ void __launch_bounds__(256)
 gh_loss_pointwise_kernel(GhLossParams prm, const float* __restrict__ out, const float* __restrict__ gt_image,
                          const float* __restrict__ gt_mask, const float* __restrict__ gt_angle,
-                         const float* __restrict__ gt_conf, double* __restrict__ sums, float* __restrict__ dL)
+                         const float* __restrict__ gt_conf, double* __restrict__ sums, float* __restrict__ dL,
+                         double* __restrict__ part)
 {
-    __shared__ double s_part[8];
     const size_t plane = (size_t)prm.W * prm.H;
     double a_l1 = 0.0, a_mask = 0.0, a_orient = 0.0;
     const float inv_sum_w = 1.0f / (float)sums[GH_LS_W];
     for (size_t pi = (size_t)blockIdx.x * 256 + threadIdx.x; pi < plane; pi += (size_t)gridDim.x * 256)
         gh_loss_pointwise(prm, plane, pi, inv_sum_w, out, gt_image, gt_mask, gt_angle, gt_conf, dL, a_l1, a_mask, a_orient);
-    gh_block_add(a_l1, sums + GH_LS_L1, s_part);
-    gh_block_add(a_mask, sums + GH_LS_MASK, s_part);
-    gh_block_add(a_orient, sums + GH_LS_ORIENT, s_part);
+    if constexpr (DET) {
+        double v[3] = {a_l1, a_mask, a_orient};
+        gh_block_sum_fixed<3>(v, part, sums, {GH_LS_L1, GH_LS_MASK, GH_LS_ORIENT}, GH_TK_POINTWISE);
+    } else {
+        __shared__ double s_part[8];
+        gh_block_add(a_l1, sums + GH_LS_L1, s_part);
+        gh_block_add(a_mask, sums + GH_LS_MASK, s_part);
+        gh_block_add(a_orient, sums + GH_LS_ORIENT, s_part);
+    }
 }
 
 // SSIM statistics of a 32x32 tile: separable 11-tap window, register blocked (a thread filters 8
 // adjacent columns of a halo row, then 4 adjacent rows of a column, so a shared-memory value is reused
 // by up to 8 taps) and paired: (x, y) and (x^2, y^2) travel as float2.
-template <int MINB>
+template <int MINB, bool DET>
 __global__ void __launch_bounds__(256, MINB)
 gh_loss_main_kernel(GhLossParams prm, const float* __restrict__ out, const float* __restrict__ gt_image,
                     const float* __restrict__ gt_mask, double* __restrict__ sums,
-                    float* __restrict__ dmaps)      // [3 channels][3 maps][H*W]
+                    float* __restrict__ dmaps,      // [3 channels][3 maps][H*W]
+                    double* __restrict__ part)
 {
     __shared__ float2 sXY[GH_LH][GH_XS];             // (x, y) = (render, target) * mask
     __shared__ float2 sH01[GH_LH][GH_HS], sH23[GH_LH][GH_HS];   // row-filtered (x, y), (x^2, y^2)
     __shared__ float sH4[GH_LH][GH_HS];              // row-filtered x y
-    __shared__ double s_part[8];
     const int W = prm.W, H = prm.H;
     const int plane = W * H;            // 10 * plane < 2^31 is checked by the host entry point
     const int tx0 = blockIdx.x * GH_LT, ty0 = blockIdx.y * GH_LT;
@@ -284,7 +370,13 @@ gh_loss_main_kernel(GhLossParams prm, const float* __restrict__ out, const float
             }
         }
     }
-    gh_block_add(a_ssim, sums + GH_LS_SSIM, s_part);
+    if constexpr (DET) {
+        double v[1] = {a_ssim};
+        gh_block_sum_fixed<1>(v, part, sums, {GH_LS_SSIM}, GH_TK_MAIN);
+    } else {
+        __shared__ double s_part[8];
+        gh_block_add(a_ssim, sums + GH_LS_SSIM, s_part);
+    }
 }
 
 template <int MINB>
@@ -429,14 +521,14 @@ extern "C" int gh_image_loss_workspace_size(int width, int height, size_t* bytes
 {
     gh_clear_error();
     if (width <= 0 || height <= 0 || !bytes) return gh_set_error(GH_E_INVALID_ARG, "gh_image_loss_workspace_size: bad width/height");
-    *bytes = GH_LS_COUNT * sizeof(double) + (size_t)9 * width * height * sizeof(float);
+    *bytes = (GH_LS_COUNT + GhLossParts::of(width, height).doubles()) * sizeof(double) + (size_t)9 * width * height * sizeof(float);
     return GH_OK;
 }
 
 extern "C" int gh_image_loss(int width, int height, const float* out_color, const float* gt_image,
                              const float* gt_mask, const float* gt_orient_angle, const float* gt_orient_conf,
                              float lambda_dl1, float lambda_dssim, float lambda_dmask, float lambda_dorient,
-                             void* workspace, float* losses, float* dL_dout, gh_stream_t stream_)
+                             void* workspace, float* losses, float* dL_dout, gh_stream_t stream_, int deterministic)
 {
     cudaStream_t stream = (cudaStream_t)stream_;
     gh_clear_error();
@@ -454,18 +546,29 @@ extern "C" int gh_image_loss(int width, int height, const float* out_color, cons
         for (int k = 0; k < 11; k++) { g[k] = (float)exp(-(double)((k - 5) * (k - 5)) / (2.0 * 1.5 * 1.5)); sum += g[k]; }
         for (int k = 0; k < 11; k++) prm.g[k] = g[k] / sum;
     }
+    const GhLossParts np = GhLossParts::of(width, height);
     double* sums = reinterpret_cast<double*>(workspace);
-    float* dmaps = reinterpret_cast<float*>(sums + GH_LS_COUNT);
+    double* part_presum = sums + GH_LS_COUNT;
+    double* part_pointwise = part_presum + np.rb;
+    double* part_main = part_pointwise + 3 * (size_t)np.pb;
+    float* dmaps = reinterpret_cast<float*>(part_main + np.mb);
     const size_t plane = (size_t)width * height;
-    if (cudaMemsetAsync(sums, 0, GH_LS_COUNT * sizeof(double), stream) != cudaSuccess)
+    if (cudaMemsetAsync(sums, 0, GH_LS_COUNT * sizeof(double), stream) != cudaSuccess)      // sums + tickets
         return gh_set_error(GH_E_CUDA, "gh_image_loss: memset of the partial sums failed");
-    const int rb = (int)((plane + 255) / 256 < 132u * 8u ? (plane + 255) / 256 : 132u * 8u);
-    gh_loss_presum_kernel<<<rb, 256, 0, stream>>>(gt_orient_conf, plane, sums);
+    const int rb = np.rb, pb = np.pb;
     const dim3 grid((width + GH_LT - 1) / GH_LT, (height + GH_LT - 1) / GH_LT), block(256);
-    const int pb = (int)((plane + 255) / 256 < 132u * 16u ? (plane + 255) / 256 : 132u * 16u);
-    gh_loss_pointwise_kernel<<<pb, 256, 0, stream>>>(prm, out_color, gt_image, gt_mask, gt_orient_angle, gt_orient_conf, sums, dL_dout);
-    // 4 CTAs per SM (64 registers)
-    gh_loss_main_kernel<4><<<grid, block, 0, stream>>>(prm, out_color, gt_image, gt_mask, sums, dmaps);
+    if (deterministic) {
+        gh_loss_presum_kernel<true><<<rb, 256, 0, stream>>>(gt_orient_conf, plane, sums, part_presum);
+        gh_loss_pointwise_kernel<true><<<pb, 256, 0, stream>>>(prm, out_color, gt_image, gt_mask, gt_orient_angle, gt_orient_conf,
+                                                               sums, dL_dout, part_pointwise);
+        gh_loss_main_kernel<4, true><<<grid, block, 0, stream>>>(prm, out_color, gt_image, gt_mask, sums, dmaps, part_main);
+    } else {
+        gh_loss_presum_kernel<false><<<rb, 256, 0, stream>>>(gt_orient_conf, plane, sums, nullptr);
+        gh_loss_pointwise_kernel<false><<<pb, 256, 0, stream>>>(prm, out_color, gt_image, gt_mask, gt_orient_angle, gt_orient_conf,
+                                                                sums, dL_dout, nullptr);
+        // 4 CTAs per SM (64 registers)
+        gh_loss_main_kernel<4, false><<<grid, block, 0, stream>>>(prm, out_color, gt_image, gt_mask, sums, dmaps, nullptr);
+    }
     gh_loss_ssim_bwd_kernel<4><<<grid, block, 0, stream>>>(prm, out_color, gt_image, gt_mask, dmaps, dL_dout);
     gh_loss_finalize_kernel<<<rb, 256, 0, stream>>>(prm, sums, losses, dL_dout);
     gh_count_launches(5);

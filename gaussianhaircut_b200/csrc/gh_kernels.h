@@ -31,6 +31,15 @@ void gh_launch_blend_backward(int W, int H, int gx, int gy, GhGeomWS geom, GhImg
                               const float* features, const float* bg, const float* dL_dpix,
                               cudaStream_t stream);
 
+// Deterministic blend backward (no atomics), three stages: the row offsets of every Gaussian (returns the number of
+// kernels launched; det.off[P] = R afterwards), the per-tile walk writing one partial row per instance, and the gather
+// that ASSIGNS geom.acc16 (no zeroing needed) by summing each Gaussian's rows in order.
+int gh_launch_det_offsets(int P, int gx, int gy, const int* radii, GhGeomWS geom, GhDetWS det, cudaStream_t stream);
+void gh_launch_blend_backward_det(int W, int H, int gx, int gy, const int* radii, GhGeomWS geom, GhImgWS img, GhBinWS bin,
+                                  GhDetWS det, const float* features, const float* bg, const float* dL_dpix,
+                                  cudaStream_t stream);
+void gh_launch_det_gather(int P, GhGeomWS geom, GhDetWS det, cudaStream_t stream);
+
 // geom.acc16 -> dL_dmean2D (P,3), dL_dconic (P,4), dL_dopacity (P), dL_dcolor (P,10); writes every row
 // (also zero-fills the geometry gradients that are non-null: used when the conic was supplied)
 void gh_launch_unpack_grads(int P, GhGeomWS geom, float* dL_dmean2D, float* dL_dconic, float* dL_dopacity,

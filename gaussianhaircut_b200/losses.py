@@ -42,7 +42,8 @@ def image_loss_forward_backward(out: torch.Tensor, gt_image: torch.Tensor, gt_ma
                                 l_dl1: float, l_dssim: float, l_dmask: float, l_dorient: float,
                                 workspace: torch.Tensor | None = None):
     """The native call itself (no autograd): returns (losses float32[8], dL_dout (10,H,W)).
-    `workspace` (float64 tensor of at least `workspace_elems(W, H)` elements) can be passed to reuse it."""
+    `workspace` (float64 tensor of at least `workspace_elems(W, H)` elements) can be passed to reuse it.
+    Under `torch.use_deterministic_algorithms(True)` the loss sums are formed in a fixed order (bit-reproducible)."""
     lib = _capi.load()
     if out.dim() != 3 or out.shape[0] != 10:
         raise RuntimeError("hair_image_loss: the render must have shape (10, H, W)")
@@ -61,7 +62,8 @@ def image_loss_forward_backward(out: torch.Tensor, gt_image: torch.Tensor, gt_ma
     with torch.cuda.device(dev):
         _capi.check(lib.gh_image_loss(W, H, _ptr(out_c), _ptr(gi), _ptr(gm), _ptr(ga), _ptr(gc),
                                       float(l_dl1), float(l_dssim), float(l_dmask), float(l_dorient),
-                                      _ptr(workspace), _ptr(losses), _ptr(dL), _stream(dev)))
+                                      _ptr(workspace), _ptr(losses), _ptr(dL), _stream(dev),
+                                      int(torch.are_deterministic_algorithms_enabled())))
     return losses, dL
 
 

@@ -137,7 +137,16 @@ int gh_forward_render(
  * When conic_precomp is given (nothing flows through the geometry), dL_dmean2D, dL_dconic, dL_dopacity and
  * dL_dcolor may ALL be NULL: the blend backward's per-Gaussian accumulation records then stay in the geometry
  * workspace for gh_project_backward to consume directly (no unpack pass).
+ *
+ * det_buffer / det_bytes select the blend backward's summation order.  det_buffer == NULL (det_bytes 0): the
+ * fast path, whose float sums depend on GPU scheduling (gradients agree run to run to ~1e-7, not bit for bit).
+ * det_buffer != NULL: the deterministic path -- no atomics, every sum in a fixed order, so every gradient is a pure
+ * function of the inputs (bit-identical across runs on the same GPU and build).  It needs det_bytes >=
+ * gh_backward_det_workspace_size(P, R) bytes of device memory; a smaller buffer, or det_bytes != 0 without a
+ * buffer, is rejected with GH_E_INVALID_ARG before anything is launched.
  */
+int gh_backward_det_workspace_size(int P, long long R, size_t* bytes);
+
 int gh_backward(
     int P, int D, int M, int R,
     int width, int height,
@@ -152,7 +161,8 @@ int gh_backward(
     const float* dL_dpix,
     float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor,
     float* dL_dmean3D, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot,
-    int debug, gh_stream_t stream);
+    int debug, gh_stream_t stream,
+    char* det_buffer, size_t det_bytes);
 
 /* Rasterizer::markVisible: present[i] = (view-space z of point i > 0.2).  `present` is bool[P]. */
 int gh_mark_visible(int P, const float* means3D, const float* viewmatrix, const float* projmatrix,
@@ -208,12 +218,15 @@ int gh_adam_step(int n_groups, float* const* params, const float* const* grads,
  * losses (device float[8]): total, Ll1, Lssim, Lmask, Lorient, sum of orientation weights,
  *   1 if Lorient was NaN (then it counts as 0 and has no gradient, like the reference), 0.
  * dL_dout (10,H,W): d total / d out_color, every element written.  No host synchronisation.
+ * deterministic != 0: the five loss sums are formed without floating-point atomics, in a fixed order (per-CTA slots
+ *   added in CTA order by the last CTA), so losses and dL_dout are bit-identical run to run; 0: one double atomicAdd
+ *   per CTA and sum, the faster path.
  */
 int gh_image_loss_workspace_size(int width, int height, size_t* bytes);
 int gh_image_loss(int width, int height, const float* out_color, const float* gt_image,
                   const float* gt_mask, const float* gt_orient_angle, const float* gt_orient_conf,
                   float lambda_dl1, float lambda_dssim, float lambda_dmask, float lambda_dorient,
-                  void* workspace, float* losses, float* dL_dout, gh_stream_t stream);
+                  void* workspace, float* losses, float* dL_dout, gh_stream_t stream, int deterministic);
 
 /*
  * Multi-GPU (SURVEY.md 8e): sum a float32 buffer that lives in SYMMETRIC memory (the same allocation on

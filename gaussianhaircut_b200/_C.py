@@ -87,19 +87,61 @@ def rasterize_gaussians(
 
         geomBuffer, imgBuffer, radii = alloc_forward_workspaces(P, W, H, device)
         out_color = torch.empty((NUM_CHANNELS, H, W), dtype=torch.float32, device=device)
-        n_rendered, max_len = C.c_int(0), C.c_int(0)
-        _capi.check(lib.gh_forward_preprocess(
+        key = (device.index, P, W, H)
+        binning, capacity = binning_hint(key)
+        stream = _stream(device)
+        n_rendered, max_len, emitted = C.c_int(0), C.c_int(0), C.c_int(0)
+        _capi.check(lib.gh_forward_preprocess_ex(
             P, int(degree), M, W, H,
             _ptr(means3D), _ptr(means2D_precomp), _ptr(sh), _ptr(colors), _ptr(opacity),
             _ptr(scales), float(scale_modifier), _ptr(rotations),
             _ptr(cov3D_precomp), _ptr(conic_precomp),
             _ptr(viewmatrix), _ptr(projmatrix), _ptr(campos),
             float(tan_fovx), float(tan_fovy), int(bool(prefiltered)),
-            _ptr(radii), _ptr(geomBuffer), _ptr(imgBuffer),
-            C.byref(n_rendered), C.byref(max_len), int(bool(debug)), _stream(device)))
+            _ptr(radii), _ptr(geomBuffer), _ptr(imgBuffer), _ptr(binning), capacity,
+            C.byref(n_rendered), C.byref(max_len), C.byref(emitted), int(bool(debug)), stream))
+        # (the GPU runs emit from here on if it fitted: keep the host's work until the second phase's launch short)
         R = int(n_rendered.value)
-        binningBuffer = _render(background, colors, radii, geomBuffer, imgBuffer, R, int(max_len.value), out_color, debug)
+        binningBuffer = _render(background, colors, radii, geomBuffer, imgBuffer, R, int(max_len.value), out_color, debug,
+                                binning if emitted.value else None, stream)
+        binning_record(key, R)
     return R, out_color, radii, geomBuffer, binningBuffer, imgBuffer
+
+
+# Capacity hint of the first phase's binning buffer: R is only known after the first phase's read-back, but the bucket
+# scatter (emit) can run behind that read-back -- while the host waits -- if the caller hands in a buffer that is large
+# enough.  Per (device, P, W, H) the R of the last few forwards is kept; the buffer is sized for their maximum plus a
+# quarter.  A first call, or an R beyond the capacity (emit then writes nothing), takes the exact-size path.
+_BIN_HISTORY = 8
+_BIN_KEYS = 64          # shapes remembered (a model that grows changes P): the oldest is dropped first
+_BIN_R: dict = {}
+
+
+def binning_capacity(key) -> int:
+    """Records the first phase's binning buffer is sized for, for a forward keyed `key` = (device index, P, W, H): the
+    largest of the last R seen for it plus a quarter (and 256 records), 0 when none has been seen."""
+    seen = _BIN_R.get(key)
+    return max(seen) + max(seen) // 4 + 256 if seen else 0
+
+
+def binning_hint(key):
+    """(binning buffer, capacity in records) for the first phase of a forward keyed `key`, or (None, 0) when no R has
+    been seen for it (binning_capacity)."""
+    capacity = binning_capacity(key)
+    if capacity == 0:
+        return None, 0
+    nbytes = C.c_size_t()
+    _capi.check(_capi.load().gh_binning_workspace_size(capacity, C.byref(nbytes)))
+    return torch.empty(nbytes.value, dtype=torch.uint8, device=torch.device("cuda", key[0])), capacity
+
+
+def binning_record(key, R: int) -> None:
+    """Remember the R of a finished first phase (see binning_hint)."""
+    if key not in _BIN_R and len(_BIN_R) >= _BIN_KEYS:
+        _BIN_R.pop(next(iter(_BIN_R)))
+    seen = _BIN_R.setdefault(key, [])
+    seen.append(int(R))
+    del seen[:-_BIN_HISTORY]
 
 
 def alloc_forward_workspaces(P: int, W: int, H: int, device: torch.device):
@@ -122,30 +164,37 @@ def alloc_forward_workspaces(P: int, W: int, H: int, device: torch.device):
 
 def forward_render(background: torch.Tensor, colors: torch.Tensor, radii: torch.Tensor, geomBuffer: torch.Tensor,
                    imgBuffer: torch.Tensor, num_rendered: int, max_tile_len: int, image_height: int, image_width: int,
-                   debug: bool = False):
+                   debug: bool = False, binned: torch.Tensor | None = None):
     """Second phase of the forward (emit, sort, blend) on workspaces whose first phase already ran
-    (gh_forward_preprocess or gh_project_forward_binned).  -> (out_color (C,H,W), binningBuffer)."""
+    (gh_forward_preprocess or gh_project_forward_binned).  `binned`: the binning buffer the first phase already
+    emitted into (projection.project_forward_binned(..., binning=True)); emit is then skipped.
+    -> (out_color (C,H,W), binningBuffer)."""
     device = colors.device
     with torch.cuda.device(device):
         out_color = torch.empty((NUM_CHANNELS, int(image_height), int(image_width)), dtype=torch.float32, device=device)
         binningBuffer = _render(_prep(background, "background", device), _prep(colors, "colors", device, align=8), radii,
-                                geomBuffer, imgBuffer, num_rendered, max_tile_len, out_color, debug)
+                                geomBuffer, imgBuffer, num_rendered, max_tile_len, out_color, debug, binned)
     return out_color, binningBuffer
 
 
-def _render(background, colors, radii, geomBuffer, imgBuffer, num_rendered, max_tile_len, out_color, debug):
-    """gh_forward_render into `out_color` on prepared tensors, inside their device's context -> binningBuffer.
-    rasterize_gaussians calls this directly: between the first phase's read-back and this launch the GPU idles."""
+def _render(background, colors, radii, geomBuffer, imgBuffer, num_rendered, max_tile_len, out_color, debug, binned=None,
+            stream=None):
+    """gh_forward_render_ex into `out_color` on prepared tensors, inside their device's context -> binningBuffer.
+    `binned`: the buffer the first phase emitted into (then used as it is), or None: a buffer of the exact size is
+    allocated and emit runs here.  `stream`: the device's current stream (_capi._stream), if the caller has it."""
     lib = _capi.load()
     device = colors.device
     H, W = int(out_color.size(1)), int(out_color.size(2))
-    bin_bytes = C.c_size_t()
-    _capi.check(lib.gh_binning_workspace_size(int(num_rendered), C.byref(bin_bytes)))
-    binningBuffer = torch.empty(bin_bytes.value, dtype=torch.uint8, device=device)
-    _capi.check(lib.gh_forward_render(
+    binningBuffer = binned
+    if binningBuffer is None:
+        bin_bytes = C.c_size_t()
+        _capi.check(lib.gh_binning_workspace_size(int(num_rendered), C.byref(bin_bytes)))
+        binningBuffer = torch.empty(bin_bytes.value, dtype=torch.uint8, device=device)
+    _capi.check(lib.gh_forward_render_ex(
         int(colors.shape[0]), W, H, _ptr(background), _ptr(colors), _ptr(radii),
         _ptr(geomBuffer), _ptr(binningBuffer), _ptr(imgBuffer),
-        int(num_rendered), int(max_tile_len), _ptr(out_color), int(bool(debug)), _stream(device)))
+        int(num_rendered), int(max_tile_len), int(binned is not None), _ptr(out_color), int(bool(debug)),
+        stream if stream is not None else _stream(device)))
     return binningBuffer
 
 

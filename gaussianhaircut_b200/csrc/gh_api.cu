@@ -8,6 +8,7 @@
 #include <cstdio>
 #include <cstring>
 #include <mutex>
+#include <string>
 
 // per-thread error message shared by every entry point of the library (gh_kernels.h)
 static thread_local char g_err[512] = "";
@@ -93,18 +94,47 @@ __global__ void gh_export_geom_kernel(int P, const GhGeo* __restrict__ geo, floa
     }
 }
 
+// The read-back of R: one thread copies ctrl into the caller's pinned host slot (mapped into the device's address space
+// under unified addressing).  A kernel rather than cudaMemcpyAsync: the copy engine's hand-offs from the tile scan and
+// back to emit cost more than the copy itself.
+__global__ void gh_ctrl_readback_kernel(const GhCtrl* __restrict__ ctrl, GhCtrl* host) { *host = *ctrl; }
+
 }  // namespace
 
 void gh_count_launches(int n) { g_launches.fetch_add((unsigned long long)n); }
 
-int gh_forward_phase1(const char* who, int P, int width, int height, char* geom_buffer, char* img_buffer, int* num_rendered,
-                      int* max_tile_len, int debug, cudaStream_t stream, GhBinLaunch launch, const void* bin)
+// The read-back target of gh_forward_phase1: one pinned slot per host thread (allocated on first use and kept for the
+// thread's lifetime; pinned memory is mapped for every device under unified addressing), so that work enqueued behind
+// the read-back runs while the host waits for it.
+static GhCtrl* gh_pinned_ctrl() {
+    static thread_local GhCtrl* slot = nullptr;
+    if (slot == nullptr && cudaMallocHost((void**)&slot, sizeof(GhCtrl)) != cudaSuccess) slot = nullptr;
+    return slot;
+}
+
+int gh_check_phase1_bin(const char* who, const GhPhase1Bin& emit)
 {
+    if (emit.capacity < 0 || emit.capacity > 0xffffffffll)
+        return gh_set_error(GH_E_INVALID_ARG, (std::string(who) + ": binning_capacity must lie in [0, 2^32)").c_str());
+    if (emit.buffer == nullptr && emit.capacity != 0)
+        return gh_set_error(GH_E_INVALID_ARG, (std::string(who) + ": binning_capacity given without a binning_buffer").c_str());
+    if (emit.buffer != nullptr && emit.emitted == nullptr)
+        return gh_set_error(GH_E_INVALID_ARG, (std::string(who) + ": a binning_buffer needs the `emitted` output").c_str());
+    return GH_OK;
+}
+
+int gh_forward_phase1(const char* who, int P, int width, int height, char* geom_buffer, char* img_buffer, int* num_rendered,
+                      int* max_tile_len, int debug, cudaStream_t stream, const GhPhase1Bin& emit, GhBinLaunch launch,
+                      const void* bin)
+{
+    if (emit.emitted) *emit.emitted = 0;
     int gx, gy; const int T = gh_tile_grid(width, height, gx, gy);
     if ((unsigned long long)gx * gx * gy >= (1ull << 32)) {    // exactness bound of the tile enumeration (gh_warp_rects)
         std::snprintf(g_err, sizeof(g_err), "%s: image too large (tile grid gx * gx * gy must stay below 2^32)", who);
         return GH_E_INVALID_ARG;
     }
+    GhCtrl* h = gh_pinned_ctrl();
+    if (h == nullptr) return gh_set_error(GH_E_CUDA, "[CUDA ERROR] cudaMallocHost(read-back slot) failed");
     GhGeomWS geom = GhGeomWS::carve(geom_buffer, (size_t)P);
     GhImgWS img = GhImgWS::carve(img_buffer, (size_t)width * height, (size_t)T);
     // ctrl + tile histogram are contiguous: one memset
@@ -118,14 +148,33 @@ int gh_forward_phase1(const char* who, int P, int width, int height, char* geom_
         g_launches += 1;
     }
     GH_STAGE(stream, debug, "tile scan");
-    GhCtrl h;
-    e = cudaMemcpyAsync(&h, img.ctrl, sizeof(GhCtrl), cudaMemcpyDeviceToHost, stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
+    cudaEvent_t ready = nullptr;
+    e = cudaEventCreateWithFlags(&ready, cudaEventDisableTiming);
+    if (e == cudaSuccess) {
+        gh_ctrl_readback_kernel<<<1, 1, 0, stream>>>(img.ctrl, h);
+        g_launches += 1;
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaEventRecord(ready, stream);
+    if (e == cudaSuccess && emit.buffer != nullptr) {
+        // emit goes in behind the read-back: it runs while the host wakes up and prepares the second phase.  It reads R
+        // from ctrl and writes nothing when the buffer is too small (the host then takes the exact-size path).
+        GhStageTimer t(GH_ST_EMIT, stream);
+        const unsigned int cap = (unsigned int)emit.capacity;
+        gh_launch_emit(P, emit.radii, geom, img, GhBinWS::carve(emit.buffer, (size_t)cap), cap, gx, gy, stream);
+        g_launches += 1;
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaEventSynchronize(ready);
+    if (ready) cudaEventDestroy(ready);
     if (e != cudaSuccess) return gh_check_cuda(e, "read back num_rendered");
-    *num_rendered = (int)h.num_rendered;
-    if (max_tile_len) *max_tile_len = (int)h.max_tile_len;
-    if (h.err_flags & GH_ERR_PREFILTERED)
+    if (emit.buffer != nullptr) GH_STAGE(stream, debug, "emit");
+    const GhCtrl hc = *h;
+    *num_rendered = (int)hc.num_rendered;
+    if (max_tile_len) *max_tile_len = (int)hc.max_tile_len;
+    if (hc.err_flags & GH_ERR_PREFILTERED)
         return gh_set_error(GH_E_PREFILTERED, "Point is filtered although prefiltered is set. This shouldn't happen!");
+    if (emit.buffer != nullptr) *emit.emitted = ((long long)hc.num_rendered <= emit.capacity) ? 1 : 0;
     return GH_OK;
 }
 
@@ -173,7 +222,7 @@ int gh_backward_det_workspace_size(int P, long long R, size_t* bytes)
     return GH_OK;
 }
 
-int gh_forward_preprocess(
+int gh_forward_preprocess_ex(
     int P, int D, int M, int width, int height,
     const float* means3D, const float* means2D_precomp, const float* shs,
     const float* colors_precomp, const float* opacities,
@@ -182,7 +231,8 @@ int gh_forward_preprocess(
     const float* viewmatrix, const float* projmatrix, const float* cam_pos,
     float tan_fovx, float tan_fovy, int prefiltered,
     int* radii, char* geom_buffer, char* img_buffer,
-    int* num_rendered, int* max_tile_len, int debug, gh_stream_t stream_)
+    char* binning_buffer, long long binning_capacity,
+    int* num_rendered, int* max_tile_len, int* emitted, int debug, gh_stream_t stream_)
 {
     (void)D; (void)M; (void)means2D_precomp; (void)shs; (void)cam_pos;
     cudaStream_t stream = (cudaStream_t)stream_;
@@ -196,8 +246,11 @@ int gh_forward_preprocess(
         return gh_set_error(GH_E_INVALID_ARG, "Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!");
     if (rotations && ((size_t)rotations & 15)) return gh_set_error(GH_E_INVALID_ARG, "rotations must be 16-byte aligned");
     if (((size_t)colors_precomp & 7)) return gh_set_error(GH_E_INVALID_ARG, "colors_precomp must be 8-byte aligned");
+    const GhPhase1Bin emit{radii, binning_buffer, binning_capacity, emitted};
+    const int rc = gh_check_phase1_bin("gh_forward_preprocess", emit);
+    if (rc != GH_OK) return rc;
     return gh_forward_phase1("gh_forward_preprocess", P, width, height, geom_buffer, img_buffer, num_rendered, max_tile_len,
-                             debug, stream, [&](const GhGeomWS& geom, const GhImgWS& img, int gx, int gy) {
+                             debug, stream, emit, [&](const GhGeomWS& geom, const GhImgWS& img, int gx, int gy) {
         GhStageTimer t(GH_ST_PREPROCESS, stream);
         gh_launch_preprocess(P, means3D, scales, scale_modifier, rotations, opacities, cov3D_precomp,
                              conic_precomp, viewmatrix, projmatrix, width, height, tan_fovx, tan_fovy,
@@ -206,11 +259,28 @@ int gh_forward_preprocess(
     });
 }
 
-int gh_forward_render(
+int gh_forward_preprocess(
+    int P, int D, int M, int width, int height,
+    const float* means3D, const float* means2D_precomp, const float* shs,
+    const float* colors_precomp, const float* opacities,
+    const float* scales, float scale_modifier, const float* rotations,
+    const float* cov3D_precomp, const float* conic_precomp,
+    const float* viewmatrix, const float* projmatrix, const float* cam_pos,
+    float tan_fovx, float tan_fovy, int prefiltered,
+    int* radii, char* geom_buffer, char* img_buffer,
+    int* num_rendered, int* max_tile_len, int debug, gh_stream_t stream_)
+{
+    return gh_forward_preprocess_ex(P, D, M, width, height, means3D, means2D_precomp, shs, colors_precomp, opacities,
+                                    scales, scale_modifier, rotations, cov3D_precomp, conic_precomp, viewmatrix, projmatrix,
+                                    cam_pos, tan_fovx, tan_fovy, prefiltered, radii, geom_buffer, img_buffer, nullptr, 0,
+                                    num_rendered, max_tile_len, nullptr, debug, stream_);
+}
+
+int gh_forward_render_ex(
     int P, int width, int height,
     const float* background, const float* colors_precomp, const int* radii,
     char* geom_buffer, char* binning_buffer, char* img_buffer,
-    int num_rendered, int max_tile_len, float* out_color, int debug, gh_stream_t stream_)
+    int num_rendered, int max_tile_len, int emitted, float* out_color, int debug, gh_stream_t stream_)
 {
     cudaStream_t stream = (cudaStream_t)stream_;
     g_err[0] = 0;
@@ -223,9 +293,9 @@ int gh_forward_render(
     GhBinWS bin = GhBinWS::carve(binning_buffer, (size_t)num_rendered);
 
     if (num_rendered > 0) {
-        {
+        if (!emitted) {
             GhStageTimer t(GH_ST_EMIT, stream);
-            gh_launch_emit(P, radii, geom, img, bin, gx, gy, stream);
+            gh_launch_emit(P, radii, geom, img, bin, (unsigned int)num_rendered, gx, gy, stream);
             g_launches += 1;
         }
         GH_STAGE(stream, debug, "emit");
@@ -242,6 +312,16 @@ int gh_forward_render(
     }
     GH_STAGE(stream, debug, "blend forward");
     return GH_OK;
+}
+
+int gh_forward_render(
+    int P, int width, int height,
+    const float* background, const float* colors_precomp, const int* radii,
+    char* geom_buffer, char* binning_buffer, char* img_buffer,
+    int num_rendered, int max_tile_len, float* out_color, int debug, gh_stream_t stream_)
+{
+    return gh_forward_render_ex(P, width, height, background, colors_precomp, radii, geom_buffer, binning_buffer, img_buffer,
+                                num_rendered, max_tile_len, 0, out_color, debug, stream_);
 }
 
 int gh_backward(

@@ -192,11 +192,15 @@ gh_tile_scan_kernel(int T, const uint32_t* __restrict__ tile_count, uint32_t* __
 // Consecutive Gaussians of a strand fall into the same tiles, so the lanes of a warp mostly ask for
 // slots of the same few buckets: lanes that want the same tile in the same loop step are grouped
 // with match.any and their leader reserves all their slots with ONE atomic.
+// `capacity`: records the instance buffer holds.  The forward's first phase may launch emit before the host has read R
+// back (gh_forward_preprocess_ex): when R = ctrl->num_rendered exceeds the capacity, no thread writes anything and the
+// tile cursors stay as the scan left them, so the host can launch emit again into a buffer of the exact size.
 __global__ void __launch_bounds__(256)
 gh_emit_kernel(int P, const int* __restrict__ radii, const GhGeo* __restrict__ geo,
                const float* __restrict__ depth, uint32_t* __restrict__ tile_cursor,
-               uint64_t* __restrict__ inst, int gx, int gy)
+               uint64_t* __restrict__ inst, int gx, int gy, const GhCtrl* __restrict__ ctrl, uint32_t capacity)
 {
+    if (ctrl->num_rendered > capacity) return;     // uniform over the grid
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;
     const int lane = threadIdx.x & 31;
     int minx = 0, miny = 0, maxx = 0, maxy = 0;
@@ -345,11 +349,11 @@ void gh_launch_tile_scan(int T, GhImgWS img, cudaStream_t stream)
     gh_tile_scan_kernel<<<GH_SCAN_CTAS, GH_SCAN_THREADS, 0, stream>>>(T, img.tile_count, img.tile_cursor, img.ranges, img.tile_perm, img.ctrl);
 }
 
-void gh_launch_emit(int P, const int* radii, GhGeomWS geom, GhImgWS img, GhBinWS bin,
+void gh_launch_emit(int P, const int* radii, GhGeomWS geom, GhImgWS img, GhBinWS bin, unsigned int capacity,
                     int gx, int gy, cudaStream_t stream)
 {
     gh_emit_kernel<<<(P + 255) / 256, 256, 0, stream>>>(P, radii, geom.geo, geom.depth,
-                                                        img.tile_cursor, bin.inst, gx, gy);
+                                                        img.tile_cursor, bin.inst, gx, gy, img.ctrl, capacity);
 }
 
 int gh_launch_tile_sort(int T, unsigned int max_tile_len, long long R, GhImgWS img, GhBinWS bin, cudaStream_t stream)

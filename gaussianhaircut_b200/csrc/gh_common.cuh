@@ -223,6 +223,49 @@ __device__ __forceinline__ GhGeo gh_geo_not_rendered() {
     return g;
 }
 
+// ---- row spans staged through shared memory (gh_preprocess_backward_kernel) ------------------------------------------
+// The rows [row0, row0 + n) of a row-major (P, K) float array are ONE contiguous span of K * n floats.  A CTA moves it
+// between global and shared memory with 16-byte accesses instead of K strided scalar accesses per thread: span element
+// i lives at s[gh_span_shift(g) + i] of a 16-byte aligned shared buffer of K * n + 4 floats, so that shared and global
+// addresses agree modulo 16 bytes; the unaligned head (< 4 floats) and tail (< 4 floats) move as scalars.  Neither the
+// span's start nor its length has to be a multiple of 4 floats.
+__device__ __forceinline__ int gh_span_shift(const float* g) { return (int)(((size_t)g >> 2) & 3u); }
+// the scalar element thread t moves: threads 0..3 the head [0, head), threads 4..7 the tail [tail0, len); -1 = none
+__device__ __forceinline__ int gh_span_edge(int t, int head, int tail0, int len) {
+    if (t < 4) return t < head ? t : -1;
+    return (t < 8 && tail0 + t - 4 < len) ? tail0 + t - 4 : -1;
+}
+
+// Issue the asynchronous copy (cp.async, LDGSTS) of the span g[0, len) into s (the shifted shared buffer above).
+// Every thread of the CTA must call it; the data is there after gh_span_wait() and a barrier.
+__device__ __forceinline__ void gh_span_load_async(float* s, const float* __restrict__ g, int len) {
+    float* sg = s + gh_span_shift(g);
+    const int head = min(len, (4 - gh_span_shift(g)) & 3);
+    const int nv = (len - head) >> 2;
+    const int i = gh_span_edge(threadIdx.x, head, head + 4 * nv, len);
+    if (i >= 0) {
+        const unsigned sa = (unsigned)__cvta_generic_to_shared(sg + i);
+        asm volatile("cp.async.ca.shared.global [%0], [%1], 4;\n" ::"r"(sa), "l"(g + i));
+    }
+    for (int i = threadIdx.x; i < nv; i += blockDim.x) {
+        const unsigned sa = (unsigned)__cvta_generic_to_shared(sg + head + 4 * i);
+        asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(sa), "l"(g + head + 4 * i));
+    }
+}
+__device__ __forceinline__ void gh_span_wait() { asm volatile("cp.async.wait_all;\n" ::: "memory"); }
+
+// Write the span g[0, len) from s (the shifted shared buffer above, complete: call after a barrier).
+__device__ __forceinline__ void gh_span_store(float* __restrict__ g, const float* s, int len) {
+    const float* sg = s + gh_span_shift(g);
+    const int head = min(len, (4 - gh_span_shift(g)) & 3);
+    const int nv = (len - head) >> 2;
+    const int i = gh_span_edge(threadIdx.x, head, head + 4 * nv, len);
+    if (i >= 0) g[i] = sg[i];
+    const float4* sv = reinterpret_cast<const float4*>(sg + head);
+    float4* gv = reinterpret_cast<float4*>(g + head);
+    for (int i = threadIdx.x; i < nv; i += blockDim.x) gv[i] = sv[i];
+}
+
 // Warp-cooperative enumeration of the (Gaussian, tile) instances of a warp's 32 tile rectangles.  Splat rectangles
 // vary a lot in size (a strand segment seen end-on covers one tile, seen sideways a dozen), so a loop in which every
 // lane walks its own rectangle runs as long as the warp's LARGEST one; here the rectangles are flattened into one

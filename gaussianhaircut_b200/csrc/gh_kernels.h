@@ -14,8 +14,8 @@ void gh_launch_mark_visible(int P, const float* means3D, const float* viewmatrix
 // exclusive scan of the tile histogram -> ranges, cursors, R, longest list
 void gh_launch_tile_scan(int T, GhImgWS img, cudaStream_t stream);
 
-// scatter (depth|idx) records into their tile buckets
-void gh_launch_emit(int P, const int* radii, GhGeomWS geom, GhImgWS img, GhBinWS bin,
+// scatter (depth|idx) records into their tile buckets; writes nothing if R (img.ctrl) exceeds `capacity` records
+void gh_launch_emit(int P, const int* radii, GhGeomWS geom, GhImgWS img, GhBinWS bin, unsigned int capacity,
                     int gx, int gy, cudaStream_t stream);
 
 // sort every tile bucket by (depth bits, gaussian idx)
@@ -56,18 +56,29 @@ void gh_launch_preprocess_backward(int P, const float* means3D, const int* radii
                                    float* dL_dmean3D, float* dL_dcov3D, float* dL_dscale, float* dL_drot,
                                    cudaStream_t stream);
 
-// The forward's first phase around its per-Gaussian kernel (gh_forward_preprocess, gh_project_forward_binned): tile grid
-// and its bound, workspace carving, ctrl + histogram memset, `bin(geom, img, gx, gy)` (launches the kernel on `stream` and
-// counts it), tile scan, read-back of R and the longest tile list.  `who` names the entry point in error messages.
+// The forward's first phase around its per-Gaussian kernel (gh_forward_preprocess[_ex], gh_project_forward_binned[_ex]):
+// tile grid and its bound, workspace carving, ctrl + histogram memset, `bin(geom, img, gx, gy)` (launches the kernel on
+// `stream` and counts it), tile scan, read-back of R and the longest tile list.  `who` names the entry point in error
+// messages.  With a binning buffer of `bin_capacity` records (`radii` then names the radii the kernel writes), emit is
+// launched right behind the read-back, so it runs while the host waits for R; *emitted tells whether R fitted.
+struct GhPhase1Bin {
+    const int* radii;          // written by the per-Gaussian kernel
+    char* buffer;              // NULL: no emit in this phase
+    long long capacity;        // records
+    int* emitted;              // out: 1 if emit ran into `buffer` (R <= capacity)
+};
 typedef void (*GhBinLaunch)(const void* bin, const GhGeomWS& geom, const GhImgWS& img, int gx, int gy);
 int gh_forward_phase1(const char* who, int P, int width, int height, char* geom_buffer, char* img_buffer, int* num_rendered,
-                      int* max_tile_len, int debug, cudaStream_t stream, GhBinLaunch launch, const void* bin);
+                      int* max_tile_len, int debug, cudaStream_t stream, const GhPhase1Bin& emit, GhBinLaunch launch,
+                      const void* bin);
 template <class F>
 int gh_forward_phase1(const char* who, int P, int width, int height, char* geom_buffer, char* img_buffer, int* num_rendered,
-                      int* max_tile_len, int debug, cudaStream_t stream, const F& bin) {
-    return gh_forward_phase1(who, P, width, height, geom_buffer, img_buffer, num_rendered, max_tile_len, debug, stream,
+                      int* max_tile_len, int debug, cudaStream_t stream, const GhPhase1Bin& emit, const F& bin) {
+    return gh_forward_phase1(who, P, width, height, geom_buffer, img_buffer, num_rendered, max_tile_len, debug, stream, emit,
                              [](const void* f, const GhGeomWS& g, const GhImgWS& i, int gx, int gy) { (*static_cast<const F*>(f))(g, i, gx, gy); }, &bin);
 }
+// argument checks of the optional binning buffer of the *_ex entry points (before any launch)
+int gh_check_phase1_bin(const char* who, const GhPhase1Bin& emit);
 
 // per-thread error message behind gh_last_error(): every extern "C" entry point clears it on entry and
 // sets it before returning a GH_E_* code (defined in gh_api.cu)

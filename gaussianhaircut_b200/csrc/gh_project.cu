@@ -345,9 +345,9 @@ extern "C" int gh_project_forward(
     return e == cudaSuccess ? GH_OK : gh_set_error(GH_E_CUDA, cudaGetErrorString(e));
 }
 
-// gh_project_forward + the rasterizer's first phase (gh_forward_phase1, as in gh_forward_preprocess) in one pass over
-// the Gaussians; continue with gh_forward_render.
-extern "C" int gh_project_forward_binned(
+// gh_project_forward + the rasterizer's first phase (gh_forward_phase1, as in gh_forward_preprocess_ex) in one pass over
+// the Gaussians; continue with gh_forward_render_ex.
+extern "C" int gh_project_forward_binned_ex(
     int P, int width, int height,
     const float* xyz, const float* scaling, const float* rotation, const float* dirs,
     const float* features_dc, const float* features_rest,
@@ -355,8 +355,8 @@ extern "C" int gh_project_forward_binned(
     const float* viewmatrix, const float* projmatrix, const float* campos,
     float tan_fovx, float tan_fovy, float scale_modifier, int sh_degree, unsigned int flags, float det_eps,
     float* means2D, float* colors, float* opacities, float* conic, float* cov3D, unsigned char* visible,
-    int* radii, char* geom_buffer, char* img_buffer, int* num_rendered, int* max_tile_len,
-    gh_stream_t stream_)
+    int* radii, char* geom_buffer, char* img_buffer, char* binning_buffer, long long binning_capacity,
+    int* num_rendered, int* max_tile_len, int* emitted, gh_stream_t stream_)
 {
     cudaStream_t stream = (cudaStream_t)stream_;
     gh_clear_error();
@@ -368,13 +368,33 @@ extern "C" int gh_project_forward_binned(
     if (!means2D || !colors || !opacities || !conic || !visible || !radii || !geom_buffer || !img_buffer || !num_rendered)
         return gh_set_error(GH_E_INVALID_ARG, "gh_project_forward_binned: missing output pointer");
     if ((size_t)colors & 7) return gh_set_error(GH_E_INVALID_ARG, "gh_project_forward_binned: colors must be 8-byte aligned");
+    const GhPhase1Bin emit{radii, binning_buffer, binning_capacity, emitted};
+    const int rc_bin = gh_check_phase1_bin("gh_project_forward_binned", emit);
+    if (rc_bin != GH_OK) return rc_bin;
     auto kernel = strand ? gh_project_forward_kernel<true, true> : gh_project_forward_kernel<true, false>;
     return gh_forward_phase1("gh_project_forward_binned", P, width, height, geom_buffer, img_buffer, num_rendered, max_tile_len,
-                             0, stream, [&](const GhGeomWS& geom, const GhImgWS& img, int gx, int gy) {
+                             0, stream, emit, [&](const GhGeomWS& geom, const GhImgWS& img, int gx, int gy) {
         kernel<<<(P + GH_PJ_THREADS - 1) / GH_PJ_THREADS, GH_PJ_THREADS, 0, stream>>>(
             A, means2D, colors, opacities, conic, cov3D, visible, radii, geom.geo, geom.depth, img.tile_count, gx, gy);
         gh_count_launches(1);
     });
+}
+
+extern "C" int gh_project_forward_binned(
+    int P, int width, int height,
+    const float* xyz, const float* scaling, const float* rotation, const float* dirs,
+    const float* features_dc, const float* features_rest,
+    const float* opacity, const float* label, const float* orient_conf,
+    const float* viewmatrix, const float* projmatrix, const float* campos,
+    float tan_fovx, float tan_fovy, float scale_modifier, int sh_degree, unsigned int flags, float det_eps,
+    float* means2D, float* colors, float* opacities, float* conic, float* cov3D, unsigned char* visible,
+    int* radii, char* geom_buffer, char* img_buffer, int* num_rendered, int* max_tile_len,
+    gh_stream_t stream_)
+{
+    return gh_project_forward_binned_ex(P, width, height, xyz, scaling, rotation, dirs, features_dc, features_rest, opacity,
+                                        label, orient_conf, viewmatrix, projmatrix, campos, tan_fovx, tan_fovy, scale_modifier,
+                                        sh_degree, flags, det_eps, means2D, colors, opacities, conic, cov3D, visible, radii,
+                                        geom_buffer, img_buffer, nullptr, 0, num_rendered, max_tile_len, nullptr, stream_);
 }
 
 extern "C" int gh_project_backward(

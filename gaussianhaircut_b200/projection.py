@@ -120,11 +120,14 @@ def project_forward(pi: ProjectionInputs, want_cov3D: bool = False, means2D_out:
     return out
 
 
-def project_forward_binned(pi: ProjectionInputs, means2D_out: Optional[torch.Tensor] = None):
+def project_forward_binned(pi: ProjectionInputs, means2D_out: Optional[torch.Tensor] = None, binning: bool = False):
     """project_forward AND the rasterizer's first phase in one pass over the Gaussians (gh_project_forward_binned):
     -> (out dict as project_forward, radii (P,) int32, geomBuffer, imgBuffer, num_rendered, max_tile_len).  Continue
     with `_C.forward_render`.  Bit-identical to project_forward followed by `_C.rasterize_gaussians` on its outputs
-    with prefiltered=False (tests/test_gpu_projection.py)."""
+    with prefiltered=False (tests/test_gpu_projection.py).
+
+    `binning=True` also runs the bucket scatter in the first phase when the capacity hint of `_C.binning_hint` covers R,
+    and appends the binning buffer it filled (or None) to the tuple: hand it to `_C.forward_render(..., binned=...)`."""
     from . import _C
     lib = _capi.load()
     dev, P = pi.device, pi.P
@@ -132,12 +135,19 @@ def project_forward_binned(pi: ProjectionInputs, means2D_out: Optional[torch.Ten
         raise RuntimeError("project_forward_binned: empty model (use project_forward + rasterize_gaussians)")
     out = alloc_outputs(P, dev, False, means2D_out)
     geom, img, radii = _C.alloc_forward_workspaces(P, int(pi.W), int(pi.H), dev)
-    n_rendered, max_len = C.c_int(0), C.c_int(0)
+    key = (dev.index, P, int(pi.W), int(pi.H))
+    buf, capacity = _C.binning_hint(key) if binning else (None, 0)
+    n_rendered, max_len, emitted = C.c_int(0), C.c_int(0), C.c_int(0)
     with torch.cuda.device(dev):
-        _capi.check(lib.gh_project_forward_binned(
+        _capi.check(lib.gh_project_forward_binned_ex(
             *_common_args(pi), _ptr(out["means2D"]), _ptr(out["colors"]), _ptr(out["opacity"]), _ptr(out["conic"]), None,
-            _ptr(out["visible"]), _ptr(radii), _ptr(geom), _ptr(img), C.byref(n_rendered), C.byref(max_len), _stream(dev)))
-    return out, radii, geom, img, int(n_rendered.value), int(max_len.value)
+            _ptr(out["visible"]), _ptr(radii), _ptr(geom), _ptr(img), _ptr(buf), capacity,
+            C.byref(n_rendered), C.byref(max_len), C.byref(emitted), _stream(dev)))
+    R = int(n_rendered.value)
+    if not binning:
+        return out, radii, geom, img, R, int(max_len.value)
+    _C.binning_record(key, R)
+    return out, radii, geom, img, R, int(max_len.value), (buf if emitted.value else None)
 
 
 _CAM_WS: Dict[tuple, torch.Tensor] = {}

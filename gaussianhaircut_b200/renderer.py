@@ -98,8 +98,9 @@ class _FusedRender(torch.autograd.Function):
         bg = st["bg"]
         if n_head == 0 and P_own > 0 and not st["debug"]:
             # one pass over the Gaussians does the projection AND the rasterizer's preprocess + tile histogram
-            out, radii, geom, img, R, max_len = projection.project_forward_binned(pi, means2D_out=viewspace.detach())
-            color, binning = _C.forward_render(bg, out["colors"], radii, geom, img, R, max_len, st["H"], st["W"])
+            out, radii, geom, img, R, max_len, binned = projection.project_forward_binned(pi, means2D_out=viewspace.detach(),
+                                                                                        binning=True)
+            color, binning = _C.forward_render(bg, out["colors"], radii, geom, img, R, max_len, st["H"], st["W"], binned=binned)
             ctx.pi, ctx.st, ctx.R, ctx.n_head, ctx.hp = pi, st, R, 0, None
             ctx.bufs = (pi.xyz, out["colors"], out["conic"], out["visible"], radii, geom, binning, img)
             ctx.mark_non_differentiable(radii)

@@ -115,6 +115,30 @@ int gh_forward_preprocess(
     int debug, gh_stream_t stream);
 
 /*
+ * gh_forward_preprocess that may also bin: given a binning buffer of gh_binning_workspace_size(binning_capacity) bytes,
+ * the bucket scatter (emit) is enqueued right behind the read-back of R, so it runs while the host waits and prepares
+ * phase 2.  *emitted = 1 if R <= binning_capacity: the buffer then holds the binned instances (pass it, with
+ * emitted = 1, to gh_forward_render_ex).  *emitted = 0 otherwise: nothing was written; size the buffer for R and call
+ * gh_forward_render_ex with emitted = 0, exactly as after gh_forward_preprocess.  binning_buffer = NULL,
+ * binning_capacity = 0 is gh_forward_preprocess.  binning_capacity must lie in [0, 2^32); `emitted` is required with a
+ * buffer.
+ */
+int gh_forward_preprocess_ex(
+    int P, int D, int M,
+    int width, int height,
+    const float* means3D, const float* means2D_precomp, const float* shs,
+    const float* colors_precomp, const float* opacities,
+    const float* scales, float scale_modifier, const float* rotations,
+    const float* cov3D_precomp, const float* conic_precomp,
+    const float* viewmatrix, const float* projmatrix, const float* cam_pos,
+    float tan_fovx, float tan_fovy, int prefiltered,
+    int* radii,
+    char* geom_buffer, char* img_buffer,
+    char* binning_buffer, long long binning_capacity,
+    int* num_rendered, int* max_tile_len, int* emitted,
+    int debug, gh_stream_t stream);
+
+/*
  * Phase 2 of Rasterizer::forward: binning + per-tile sort + front-to-back blend.
  * out_color is (C, H, W) channel-major, fully overwritten (background included).
  */
@@ -124,6 +148,16 @@ int gh_forward_render(
     const int* radii,
     char* geom_buffer, char* binning_buffer, char* img_buffer,
     int num_rendered, int max_tile_len,
+    float* out_color,
+    int debug, gh_stream_t stream);
+/* gh_forward_render; emitted = 1 skips the bucket scatter that the first phase already ran into binning_buffer
+ * (gh_forward_preprocess_ex / gh_project_forward_binned_ex reported *emitted = 1 for this buffer). */
+int gh_forward_render_ex(
+    int P, int width, int height,
+    const float* background, const float* colors_precomp,
+    const int* radii,
+    char* geom_buffer, char* binning_buffer, char* img_buffer,
+    int num_rendered, int max_tile_len, int emitted,
     float* out_color,
     int debug, gh_stream_t stream);
 
@@ -312,6 +346,18 @@ int gh_project_forward_binned(
     float tan_fovx, float tan_fovy, float scale_modifier, int sh_degree, unsigned int flags, float det_eps,
     float* means2D, float* colors, float* opacities, float* conic, float* cov3D, unsigned char* visible,
     int* radii, char* geom_buffer, char* img_buffer, int* num_rendered, int* max_tile_len,
+    gh_stream_t stream);
+/* gh_project_forward_binned with the optional binning buffer of gh_forward_preprocess_ex (same contract). */
+int gh_project_forward_binned_ex(
+    int P, int width, int height,
+    const float* xyz, const float* scaling, const float* rotation, const float* dirs,
+    const float* features_dc, const float* features_rest,
+    const float* opacity, const float* label, const float* orient_conf,
+    const float* viewmatrix, const float* projmatrix, const float* campos,
+    float tan_fovx, float tan_fovy, float scale_modifier, int sh_degree, unsigned int flags, float det_eps,
+    float* means2D, float* colors, float* opacities, float* conic, float* cov3D, unsigned char* visible,
+    int* radii, char* geom_buffer, char* img_buffer, char* binning_buffer, long long binning_capacity,
+    int* num_rendered, int* max_tile_len, int* emitted,
     gh_stream_t stream);
 int gh_project_backward(
     int P, int width, int height,

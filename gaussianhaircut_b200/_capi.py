@@ -122,6 +122,9 @@ SIGNATURES = {
     "gh_densify_classify": (_i, [_i, _p, _p, _p, _p, _f, _f, _f, _f, _p, _p]),
     "gh_densify_scatter": (_i, [_i, _i, _p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _p, _p, _i, _i, _i, _p, _i, _p]),
     "gh_debug_export": (_i, [_i, _i, _i, _ll, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "gh_knn_workspace_size": (_i, [_ll, C.POINTER(_sz)]),
+    "gh_knn_morton": (_i, [_ll, _p, _p, _p, _sz, _p]),                # P points codes workspace bytes stream
+    "gh_knn_mean_dist3": (_i, [_ll, _p, _p, _p, _p, _sz, _p]),        # P points order out workspace bytes stream
 }
 
 _lib = None

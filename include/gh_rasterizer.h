@@ -414,6 +414,27 @@ int gh_densify_scatter(int P, int n_tensors, const float* const* src, const floa
                        const int* flags, const int* inclusive_prefix, int n_keep, int n_clone, int n_split_kept,
                        const float* samples, int n_split_all, gh_stream_t stream);
 
+/*
+ * Exact 3-nearest-neighbour mean squared distance of a point cloud (the reference's `simple_knn._C.distCUDA2`,
+ * called by GaussianModel.create_from_pcd, src/scene/gaussian_model.py:409, to size the initial Gaussians).
+ * points (P,3) float32, 4-byte aligned; P in [0, 2^31).  For every point i with finite coordinates,
+ *   out[i] = ((b0 + b1) + b2) / 3,  b0 <= b1 <= b2 the three smallest of s_j = (dx*dx + dy*dy) + dz*dz,
+ *   dx = p_j.x - p_i.x, ..., over the finite points j != i (told apart by index: a duplicate is at distance 0), every
+ *   operation rounded on its own; slots without a candidate are +inf (P <= 3 gives +inf).  A point with a NaN or
+ *   infinite coordinate gets NaN and is nobody's neighbour.  The result depends only on the multiset of distances.
+ * Two calls with the same workspace of gh_knn_workspace_size(P) bytes (any alignment; device memory), on one stream:
+ *   gh_knn_morton: codes (P) int64, 8-byte aligned = 63-bit Morton codes of the finite points on their bounding box,
+ *     INT64_MAX for the others;
+ *   the caller sorts the codes: order (P) int64 = the permutation that sorts them (torch.sort(..., stable=True));
+ *   gh_knn_mean_dist3: out (P) float32.  `order` must be a permutation of [0, P); an entry outside it is skipped.
+ *     Any permutation gives the same result: the order only decides how fast the search prunes.
+ * No host synchronisation; P = 0 launches nothing.
+ */
+int gh_knn_workspace_size(long long P, size_t* bytes);
+int gh_knn_morton(long long P, const float* points, long long* codes, void* workspace, size_t bytes, gh_stream_t stream);
+int gh_knn_mean_dist3(long long P, const float* points, const long long* order, float* out, void* workspace,
+                      size_t bytes, gh_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -125,6 +125,9 @@ SIGNATURES = {
     "gh_knn_workspace_size": (_i, [_ll, C.POINTER(_sz)]),
     "gh_knn_morton": (_i, [_ll, _p, _p, _p, _sz, _p]),                # P points codes workspace bytes stream
     "gh_knn_mean_dist3": (_i, [_ll, _p, _p, _p, _p, _sz, _p]),        # P points order out workspace bytes stream
+    "gh_orient_workspace_size": (_i, [_i, _i, _i, _i, _i, C.POINTER(_sz)]),   # H W N K num_filters bytes
+    "gh_orient_dog": (_i, [_i, _i, _i, _p, _p, _i, _p, _i, _p, _p, _sz, _p]),  # H W C image w_low r_low w_high r_high dog ws bytes stream
+    "gh_orient_gabor": (_i, [_i, _i, _p, _i, _i, _i, _p, _p, _p, _p, _sz, _p]),  # H W bank N K nf thetas orients var ws bytes stream
 }
 
 _lib = None

@@ -435,6 +435,36 @@ int gh_knn_morton(long long P, const float* points, long long* codes, void* work
 int gh_knn_mean_dist3(long long P, const float* points, const long long* order, float* out, void* workspace,
                       size_t bytes, gh_stream_t stream);
 
+/*
+ * Hair orientation maps (the reference's `calc_orients`, src/preprocessing/calc_orientation_maps.py:53-97, evaluated on
+ * the whole image; DESIGN §15).  Image (H,W,C) uint8, C = 3 (RGB) or 4 (RGBA, alpha ignored), row-major.
+ *   gray = 0.2989 r + 0.5870 g + 0.1140 b (float64);
+ *   dog (H,W) float64 = G(gray, w_low) - G(gray, w_high), G = the separable Gaussian of scipy.ndimage.gaussian_filter
+ *     (axis 0 first, mode 'nearest'), each axis with correlate1d's symmetric order: x[i] w[r], then
+ *     + (x[i+jj] + x[i-jj]) w[r+jj] for jj = -r .. -1.  w_* (2r+1) float64 device arrays = the normalised weights
+ *     exp(-0.5 / s^2 * x^2) / sum, r = int(4 s + 0.5) (the caller computes them, as scipy does, on the host);
+ *   bank (N,K,K) float32 = the real Gabor filters in theta-major order c = j*G + g (j < num_filters, G = N/num_filters),
+ *     each zero-padded to the centre of the odd K x K square; thetas (num_filters) float32;
+ *   R_c(y,x) = sum_{ky,kx} bank[c][ky][kx] * float32(dog)[y+ky-K/2][x+kx-K/2] (cross-correlation, zero outside the
+ *     image) in FP32 FMA; F_j = |R_{j*G+g}|; per group idx_g = argmax_j F_j (first on ties), var_g = the float32
+ *     epilogue of gaussianhaircut_b200/csrc/gh_orient_math.h; orients (H,W) int64 = idx of the first group with the
+ *     smallest var_g, var (H,W) float32 = that var_g.
+ * One workspace of gh_orient_workspace_size(H, W, N, K, num_filters) bytes, 256-byte aligned device memory, serves both
+ * calls in order on one stream: gh_orient_dog leaves float32(dog) in it for gh_orient_gabor.  Caps: odd K <=
+ * GH_ORIENT_MAX_K, num_filters <= GH_ORIENT_MAX_FILTERS, N <= GH_ORIENT_MAX_N, radii <= GH_ORIENT_MAX_RADIUS; H, W > 0
+ * with H*W < 2^31.  Bad arguments are rejected before any launch.  No host synchronisation, no atomics: the maps are
+ * bit-reproducible.
+ */
+#define GH_ORIENT_MAX_K 17
+#define GH_ORIENT_MAX_FILTERS 256
+#define GH_ORIENT_MAX_N 4096
+#define GH_ORIENT_MAX_RADIUS 4096
+int gh_orient_workspace_size(int H, int W, int N, int K, int num_filters, size_t* bytes);
+int gh_orient_dog(int H, int W, int C, const unsigned char* image, const double* w_low, int r_low,
+                  const double* w_high, int r_high, double* dog, void* workspace, size_t bytes, gh_stream_t stream);
+int gh_orient_gabor(int H, int W, const float* bank, int N, int K, int num_filters, const float* thetas,
+                    long long* orients, float* var, void* workspace, size_t bytes, gh_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -91,7 +91,7 @@ def rasterize_gaussians(
         binning, capacity = binning_hint(key)
         stream = _stream(device)
         n_rendered, max_len, emitted = C.c_int(0), C.c_int(0), C.c_int(0)
-        _capi.check(lib.gh_forward_preprocess_ex(
+        _capi.check(lib.gh_forward_preprocess(
             P, int(degree), M, W, H,
             _ptr(means3D), _ptr(means2D_precomp), _ptr(sh), _ptr(colors), _ptr(opacity),
             _ptr(scales), float(scale_modifier), _ptr(rotations),
@@ -179,7 +179,7 @@ def forward_render(background: torch.Tensor, colors: torch.Tensor, radii: torch.
 
 def _render(background, colors, radii, geomBuffer, imgBuffer, num_rendered, max_tile_len, out_color, debug, binned=None,
             stream=None):
-    """gh_forward_render_ex into `out_color` on prepared tensors, inside their device's context -> binningBuffer.
+    """gh_forward_render into `out_color` on prepared tensors, inside their device's context -> binningBuffer.
     `binned`: the buffer the first phase emitted into (then used as it is), or None: a buffer of the exact size is
     allocated and emit runs here.  `stream`: the device's current stream (_capi._stream), if the caller has it."""
     lib = _capi.load()
@@ -190,7 +190,7 @@ def _render(background, colors, radii, geomBuffer, imgBuffer, num_rendered, max_
         bin_bytes = C.c_size_t()
         _capi.check(lib.gh_binning_workspace_size(int(num_rendered), C.byref(bin_bytes)))
         binningBuffer = torch.empty(bin_bytes.value, dtype=torch.uint8, device=device)
-    _capi.check(lib.gh_forward_render_ex(
+    _capi.check(lib.gh_forward_render(
         int(colors.shape[0]), W, H, _ptr(background), _ptr(colors), _ptr(radii),
         _ptr(geomBuffer), _ptr(binningBuffer), _ptr(imgBuffer),
         int(num_rendered), int(max_tile_len), int(binned is not None), _ptr(out_color), int(bool(debug)),

@@ -22,7 +22,7 @@ GH_E_NO_COLORS = 2
 GH_E_CUDA = 3
 GH_E_PREFILTERED = 4
 
-ABI_VERSION = 4
+ABI_VERSION = 5
 
 _p = C.c_void_p
 _i = C.c_int
@@ -59,23 +59,10 @@ SIGNATURES = {
         _f, _f, _i,                          # tan_fovx tan_fovy prefiltered
         _p,                                  # radii
         _p, _p,                              # geom_buffer img_buffer
-        C.POINTER(_i), C.POINTER(_i),        # num_rendered max_tile_len
-        _i, _p]),                            # debug stream
-    "gh_forward_preprocess_ex": (_i, [
-        _i, _i, _i, _i, _i,                  # P D M width height
-        _p, _p, _p, _p, _p,                  # means3D means2D_precomp shs colors_precomp opacities
-        _p, _f, _p,                          # scales scale_modifier rotations
-        _p, _p,                              # cov3D_precomp conic_precomp
-        _p, _p, _p,                          # viewmatrix projmatrix cam_pos
-        _f, _f, _i,                          # tan_fovx tan_fovy prefiltered
-        _p,                                  # radii
-        _p, _p,                              # geom_buffer img_buffer
         _p, _ll,                             # binning_buffer binning_capacity (records)
         C.POINTER(_i), C.POINTER(_i), C.POINTER(_i),   # num_rendered max_tile_len emitted
         _i, _p]),                            # debug stream
     "gh_forward_render": (_i, [
-        _i, _i, _i, _p, _p, _p, _p, _p, _p, _i, _i, _p, _i, _p]),
-    "gh_forward_render_ex": (_i, [
         _i, _i, _i, _p, _p, _p, _p, _p, _p, _i, _i, _i, _p, _i, _p]),     # ... num_rendered max_tile_len emitted ...
     "gh_backward": (_i, [
         _i, _i, _i, _i, _i, _i,              # P D M R width height
@@ -102,10 +89,6 @@ SIGNATURES = {
         _p, _p, _p, _p, _p, _p,              # means2D colors opacities conic cov3D visible
         _p]),                                # stream
     "gh_project_forward_binned": (_i, _PROJ_ARGS + [
-        _p, _p, _p, _p, _p, _p,              # means2D colors opacities conic cov3D visible
-        _p, _p, _p, C.POINTER(C.c_int), C.POINTER(C.c_int),   # radii geom_buffer img_buffer num_rendered max_tile_len
-        _p]),
-    "gh_project_forward_binned_ex": (_i, _PROJ_ARGS + [
         _p, _p, _p, _p, _p, _p,              # means2D colors opacities conic cov3D visible
         _p, _p, _p, _p, _ll,                 # radii geom_buffer img_buffer binning_buffer binning_capacity
         C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int),   # num_rendered max_tile_len emitted

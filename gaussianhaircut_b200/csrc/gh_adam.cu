@@ -149,13 +149,10 @@ extern "C" int gh_adam_step(int n_groups, float* const* params, const float* con
     const unsigned long long want = (largest / 4 + 255) / 256;
     const dim3 grid((unsigned int)(want < 1 ? 1 : (want > 132ull * 8 ? 132ull * 8 : want)), (unsigned int)n_groups);
     if (nan_flag) {
-        if (cudaMemsetAsync(nan_flag, 0, sizeof(unsigned int), stream) != cudaSuccess)
-            return gh_set_error(GH_E_CUDA, "gh_adam_step: memset of the NaN flag failed");
+        const cudaError_t e = cudaMemsetAsync(nan_flag, 0, sizeof(unsigned int), stream);
+        if (e != cudaSuccess) return gh_cuda_status("gh_adam_step", "memset(NaN flag)", e);
         gh_adam_nan_kernel<<<grid, 256, 0, stream>>>(g, nan_flag);
-        gh_count_launches(1);
     }
     gh_adam_update_kernel<<<grid, 256, 0, stream>>>(g, beta1, beta2, eps, (float)bc1, (float)sqrt(bc2), nan_flag, skip_flag, step_state);
-    gh_count_launches(1);
-    const cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? GH_OK : gh_set_error(GH_E_CUDA, cudaGetErrorString(e));
+    return gh_launch_status("gh_adam_step", nan_flag ? 2 : 1);
 }

@@ -243,8 +243,9 @@ extern "C" int gh_allreduce_p2p(const unsigned long long* peer_bufs, const unsig
     const int max_ctas = gh_env_int("GH_ALLREDUCE_MAX_CTAS", 1 << 20, 1, 1 << 20);
     const unsigned long long timeout_ns = 1000000ull * (unsigned long long)gh_env_int("GH_ALLREDUCE_TIMEOUT_MS", 30000, 1, 3600000);
     int dev = 0, sms = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
-        return gh_set_error(GH_E_CUDA, "gh_allreduce_p2p: cannot query the device");
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    if (e != cudaSuccess) return gh_cuda_status("gh_allreduce_p2p", "query the device", e);
     const size_t n4 = n_floats / 4, per_rank = (n4 + world - 1) / world;
 
 #define GH_AR_LAUNCH(WT, MU)                                                                                       \
@@ -271,7 +272,5 @@ extern "C" int gh_allreduce_p2p(const unsigned long long* peer_bufs, const unsig
     else if (world == 8) GH_AR_LAUNCH(8, 1);
     else GH_AR_LAUNCH(0, 1);
 #undef GH_AR_LAUNCH
-    gh_count_launches(1);
-    const cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? GH_OK : gh_set_error(GH_E_CUDA, cudaGetErrorString(e));
+    return gh_launch_status("gh_allreduce_p2p", 1);
 }

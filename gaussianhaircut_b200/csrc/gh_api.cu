@@ -5,33 +5,33 @@
 #include "../../include/gh_rasterizer.h"
 
 #include <atomic>
+#include <cstdarg>
 #include <cstdio>
 #include <cstring>
 #include <mutex>
-#include <string>
 
 // per-thread error message shared by every entry point of the library (gh_kernels.h)
 static thread_local char g_err[512] = "";
 void gh_clear_error() { g_err[0] = 0; }
-int gh_set_error(int code, const char* msg) {
-    std::snprintf(g_err, sizeof(g_err), "%s", msg ? msg : "");
+int gh_set_error(int code, const char* fmt, ...) {
+    va_list ap;
+    va_start(ap, fmt);
+    std::vsnprintf(g_err, sizeof(g_err), fmt, ap);
+    va_end(ap);
     return code;
+}
+int gh_cuda_status(const char* who, const char* what, cudaError_t e) {
+    return e == cudaSuccess ? GH_OK : gh_set_error(GH_E_CUDA, "[CUDA ERROR] %s: %s: %s", who, what, cudaGetErrorString(e));
 }
 
 namespace {
 
-int gh_check_cuda(cudaError_t e, const char* what) {
-    if (e == cudaSuccess) return GH_OK;
-    std::snprintf(g_err, sizeof(g_err), "[CUDA ERROR] %s: %s", what, cudaGetErrorString(e));
-    return GH_E_CUDA;
-}
-
 // debug mode mirrors the reference's CHECK_CUDA (auxiliary.h:166-173): sync + report after each stage
-#define GH_STAGE(stream, debug, what)                                             \
+#define GH_STAGE(who, stream, debug, what)                                        \
     do {                                                                           \
         cudaError_t e__ = cudaGetLastError();                                      \
         if (e__ == cudaSuccess && (debug)) e__ = cudaStreamSynchronize(stream);    \
-        if (e__ != cudaSuccess) return gh_check_cuda(e__, what);                   \
+        if (e__ != cudaSuccess) return gh_cuda_status(who, what, e__);             \
     } while (0)
 
 // ---- optional per-stage device timing (bench / roofline only; off by default) -------------------
@@ -103,23 +103,31 @@ __global__ void gh_ctrl_readback_kernel(const GhCtrl* __restrict__ ctrl, GhCtrl*
 
 void gh_count_launches(int n) { g_launches.fetch_add((unsigned long long)n); }
 
+int gh_launch_status(const char* who, int n) {
+    gh_count_launches(n);
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? GH_OK : gh_set_error(GH_E_CUDA, "[CUDA ERROR] %s: %s", who, cudaGetErrorString(e));
+}
+
 // The read-back target of gh_forward_phase1: one pinned slot per host thread (allocated on first use and kept for the
 // thread's lifetime; pinned memory is mapped for every device under unified addressing), so that work enqueued behind
 // the read-back runs while the host waits for it.
-static GhCtrl* gh_pinned_ctrl() {
+static cudaError_t gh_pinned_ctrl(GhCtrl** out) {
     static thread_local GhCtrl* slot = nullptr;
-    if (slot == nullptr && cudaMallocHost((void**)&slot, sizeof(GhCtrl)) != cudaSuccess) slot = nullptr;
-    return slot;
+    const cudaError_t e = slot != nullptr ? cudaSuccess : cudaMallocHost((void**)&slot, sizeof(GhCtrl));
+    if (e != cudaSuccess) slot = nullptr;
+    *out = slot;
+    return e;
 }
 
 int gh_check_phase1_bin(const char* who, const GhPhase1Bin& emit)
 {
     if (emit.capacity < 0 || emit.capacity > 0xffffffffll)
-        return gh_set_error(GH_E_INVALID_ARG, (std::string(who) + ": binning_capacity must lie in [0, 2^32)").c_str());
+        return gh_set_error(GH_E_INVALID_ARG, "%s: binning_capacity must lie in [0, 2^32)", who);
     if (emit.buffer == nullptr && emit.capacity != 0)
-        return gh_set_error(GH_E_INVALID_ARG, (std::string(who) + ": binning_capacity given without a binning_buffer").c_str());
+        return gh_set_error(GH_E_INVALID_ARG, "%s: binning_capacity given without a binning_buffer", who);
     if (emit.buffer != nullptr && emit.emitted == nullptr)
-        return gh_set_error(GH_E_INVALID_ARG, (std::string(who) + ": a binning_buffer needs the `emitted` output").c_str());
+        return gh_set_error(GH_E_INVALID_ARG, "%s: a binning_buffer needs the `emitted` output", who);
     return GH_OK;
 }
 
@@ -129,46 +137,43 @@ int gh_forward_phase1(const char* who, int P, int width, int height, char* geom_
 {
     if (emit.emitted) *emit.emitted = 0;
     int gx, gy; const int T = gh_tile_grid(width, height, gx, gy);
-    if ((unsigned long long)gx * gx * gy >= (1ull << 32)) {    // exactness bound of the tile enumeration (gh_warp_rects)
-        std::snprintf(g_err, sizeof(g_err), "%s: image too large (tile grid gx * gx * gy must stay below 2^32)", who);
-        return GH_E_INVALID_ARG;
-    }
-    GhCtrl* h = gh_pinned_ctrl();
-    if (h == nullptr) return gh_set_error(GH_E_CUDA, "[CUDA ERROR] cudaMallocHost(read-back slot) failed");
+    if ((unsigned long long)gx * gx * gy >= (1ull << 32))      // exactness bound of the tile enumeration (gh_warp_rects)
+        return gh_set_error(GH_E_INVALID_ARG, "%s: image too large (tile grid gx * gx * gy must stay below 2^32)", who);
+    GhCtrl* h = nullptr;
+    int rc = gh_cuda_status(who, "cudaMallocHost(read-back slot)", gh_pinned_ctrl(&h));
+    if (rc != GH_OK) return rc;
     GhGeomWS geom = GhGeomWS::carve(geom_buffer, (size_t)P);
     GhImgWS img = GhImgWS::carve(img_buffer, (size_t)width * height, (size_t)T);
     // ctrl + tile histogram are contiguous: one memset
-    cudaError_t e = cudaMemsetAsync(img.ctrl, 0, 256 + gh_align_up((size_t)T * 4, 256), stream);
-    if (e != cudaSuccess) return gh_check_cuda(e, "memset(tile histogram)");
+    rc = gh_cuda_status(who, "memset(tile histogram)", cudaMemsetAsync(img.ctrl, 0, 256 + gh_align_up((size_t)T * 4, 256), stream));
+    if (rc != GH_OK) return rc;
     launch(bin, geom, img, gx, gy);
-    GH_STAGE(stream, debug, "preprocess");
+    GH_STAGE(who, stream, debug, "preprocess");
     {
         GhStageTimer t(GH_ST_TILE_SCAN, stream);
         gh_launch_tile_scan(T, img, stream);
         g_launches += 1;
     }
-    GH_STAGE(stream, debug, "tile scan");
+    GH_STAGE(who, stream, debug, "tile scan");
     cudaEvent_t ready = nullptr;
-    e = cudaEventCreateWithFlags(&ready, cudaEventDisableTiming);
-    if (e == cudaSuccess) {
+    rc = gh_cuda_status(who, "create the read-back event", cudaEventCreateWithFlags(&ready, cudaEventDisableTiming));
+    if (rc == GH_OK) {
         gh_ctrl_readback_kernel<<<1, 1, 0, stream>>>(img.ctrl, h);
-        g_launches += 1;
-        e = cudaGetLastError();
+        rc = gh_launch_status(who, 1);
     }
-    if (e == cudaSuccess) e = cudaEventRecord(ready, stream);
-    if (e == cudaSuccess && emit.buffer != nullptr) {
+    if (rc == GH_OK) rc = gh_cuda_status(who, "record the read-back event", cudaEventRecord(ready, stream));
+    if (rc == GH_OK && emit.buffer != nullptr) {
         // emit goes in behind the read-back: it runs while the host wakes up and prepares the second phase.  It reads R
         // from ctrl and writes nothing when the buffer is too small (the host then takes the exact-size path).
         GhStageTimer t(GH_ST_EMIT, stream);
         const unsigned int cap = (unsigned int)emit.capacity;
         gh_launch_emit(P, emit.radii, geom, img, GhBinWS::carve(emit.buffer, (size_t)cap), cap, gx, gy, stream);
-        g_launches += 1;
-        e = cudaGetLastError();
+        rc = gh_launch_status(who, 1);
     }
-    if (e == cudaSuccess) e = cudaEventSynchronize(ready);
+    if (rc == GH_OK) rc = gh_cuda_status(who, "read back num_rendered", cudaEventSynchronize(ready));
     if (ready) cudaEventDestroy(ready);
-    if (e != cudaSuccess) return gh_check_cuda(e, "read back num_rendered");
-    if (emit.buffer != nullptr) GH_STAGE(stream, debug, "emit");
+    if (rc != GH_OK) return rc;
+    if (emit.buffer != nullptr) GH_STAGE(who, stream, debug, "emit");
     const GhCtrl hc = *h;
     *num_rendered = (int)hc.num_rendered;
     if (max_tile_len) *max_tile_len = (int)hc.max_tile_len;
@@ -180,7 +185,7 @@ int gh_forward_phase1(const char* who, int P, int width, int height, char* geom_
 
 extern "C" {
 
-int gh_abi_version(void) { return 4; }
+int gh_abi_version(void) { return 5; }
 
 unsigned long long gh_kernel_launch_count(void) { return g_launches.load(); }
 
@@ -201,6 +206,7 @@ const char* gh_last_error(void) { return g_err; }
 
 int gh_forward_workspace_sizes(int P, int width, int height, size_t* geom_bytes, size_t* img_bytes)
 {
+    gh_clear_error();
     if (P < 0 || width <= 0 || height <= 0) return gh_set_error(GH_E_INVALID_ARG, "gh_forward_workspace_sizes: bad P/width/height");
     int gx, gy; gh_tile_grid(width, height, gx, gy);
     if (geom_bytes) *geom_bytes = GhGeomWS::bytes((size_t)P);
@@ -210,6 +216,7 @@ int gh_forward_workspace_sizes(int P, int width, int height, size_t* geom_bytes,
 
 int gh_binning_workspace_size(long long R, size_t* binning_bytes)
 {
+    gh_clear_error();
     if (R < 0) return gh_set_error(GH_E_INVALID_ARG, "gh_binning_workspace_size: negative R");
     if (binning_bytes) *binning_bytes = GhBinWS::bytes((size_t)R);
     return GH_OK;
@@ -217,12 +224,13 @@ int gh_binning_workspace_size(long long R, size_t* binning_bytes)
 
 int gh_backward_det_workspace_size(int P, long long R, size_t* bytes)
 {
+    gh_clear_error();
     if (P < 0 || R < 0 || R > 0xffffffffll) return gh_set_error(GH_E_INVALID_ARG, "gh_backward_det_workspace_size: bad P/R");
     if (bytes) *bytes = GhDetWS::bytes((size_t)P, (size_t)R);
     return GH_OK;
 }
 
-int gh_forward_preprocess_ex(
+int gh_forward_preprocess(
     int P, int D, int M, int width, int height,
     const float* means3D, const float* means2D_precomp, const float* shs,
     const float* colors_precomp, const float* opacities,
@@ -236,7 +244,7 @@ int gh_forward_preprocess_ex(
 {
     (void)D; (void)M; (void)means2D_precomp; (void)shs; (void)cam_pos;
     cudaStream_t stream = (cudaStream_t)stream_;
-    g_err[0] = 0;
+    gh_clear_error();
     if (P <= 0 || width <= 0 || height <= 0) return gh_set_error(GH_E_INVALID_ARG, "gh_forward_preprocess: P, width, height must be positive");
     if (colors_precomp == nullptr)
         return gh_set_error(GH_E_NO_COLORS, "For non-RGB, provide precomputed Gaussian colors!");
@@ -259,31 +267,14 @@ int gh_forward_preprocess_ex(
     });
 }
 
-int gh_forward_preprocess(
-    int P, int D, int M, int width, int height,
-    const float* means3D, const float* means2D_precomp, const float* shs,
-    const float* colors_precomp, const float* opacities,
-    const float* scales, float scale_modifier, const float* rotations,
-    const float* cov3D_precomp, const float* conic_precomp,
-    const float* viewmatrix, const float* projmatrix, const float* cam_pos,
-    float tan_fovx, float tan_fovy, int prefiltered,
-    int* radii, char* geom_buffer, char* img_buffer,
-    int* num_rendered, int* max_tile_len, int debug, gh_stream_t stream_)
-{
-    return gh_forward_preprocess_ex(P, D, M, width, height, means3D, means2D_precomp, shs, colors_precomp, opacities,
-                                    scales, scale_modifier, rotations, cov3D_precomp, conic_precomp, viewmatrix, projmatrix,
-                                    cam_pos, tan_fovx, tan_fovy, prefiltered, radii, geom_buffer, img_buffer, nullptr, 0,
-                                    num_rendered, max_tile_len, nullptr, debug, stream_);
-}
-
-int gh_forward_render_ex(
+int gh_forward_render(
     int P, int width, int height,
     const float* background, const float* colors_precomp, const int* radii,
     char* geom_buffer, char* binning_buffer, char* img_buffer,
     int num_rendered, int max_tile_len, int emitted, float* out_color, int debug, gh_stream_t stream_)
 {
     cudaStream_t stream = (cudaStream_t)stream_;
-    g_err[0] = 0;
+    gh_clear_error();
     if (P <= 0 || width <= 0 || height <= 0 || num_rendered < 0) return gh_set_error(GH_E_INVALID_ARG, "gh_forward_render: bad sizes");
     if (!background || !colors_precomp || !radii || !geom_buffer || !img_buffer || !out_color || (num_rendered > 0 && !binning_buffer))
         return gh_set_error(GH_E_INVALID_ARG, "gh_forward_render: missing mandatory pointer");
@@ -298,30 +289,20 @@ int gh_forward_render_ex(
             gh_launch_emit(P, radii, geom, img, bin, (unsigned int)num_rendered, gx, gy, stream);
             g_launches += 1;
         }
-        GH_STAGE(stream, debug, "emit");
+        GH_STAGE("gh_forward_render", stream, debug, "emit");
         {
             GhStageTimer t(GH_ST_TILE_SORT, stream);
             g_launches += gh_launch_tile_sort(T, (unsigned int)max_tile_len, (long long)num_rendered, img, bin, stream);
         }
-        GH_STAGE(stream, debug, "tile sort");
+        GH_STAGE("gh_forward_render", stream, debug, "tile sort");
     }
     {
         GhStageTimer t(GH_ST_BLEND_FWD, stream);
         gh_launch_blend_forward(width, height, gx, gy, geom, img, bin, colors_precomp, background, out_color, stream);
         g_launches += 1;
     }
-    GH_STAGE(stream, debug, "blend forward");
+    GH_STAGE("gh_forward_render", stream, debug, "blend forward");
     return GH_OK;
-}
-
-int gh_forward_render(
-    int P, int width, int height,
-    const float* background, const float* colors_precomp, const int* radii,
-    char* geom_buffer, char* binning_buffer, char* img_buffer,
-    int num_rendered, int max_tile_len, float* out_color, int debug, gh_stream_t stream_)
-{
-    return gh_forward_render_ex(P, width, height, background, colors_precomp, radii, geom_buffer, binning_buffer, img_buffer,
-                                num_rendered, max_tile_len, 0, out_color, debug, stream_);
 }
 
 int gh_backward(
@@ -340,7 +321,7 @@ int gh_backward(
 {
     (void)D; (void)M; (void)shs; (void)campos; (void)dL_dsh;
     cudaStream_t stream = (cudaStream_t)stream_;
-    g_err[0] = 0;
+    gh_clear_error();
     if (P <= 0 || width <= 0 || height <= 0 || R < 0) return gh_set_error(GH_E_INVALID_ARG, "gh_backward: bad sizes");
     if (det_buffer == nullptr && det_bytes != 0)
         return gh_set_error(GH_E_INVALID_ARG, "gh_backward: det_bytes given without a det_buffer");
@@ -371,7 +352,7 @@ int gh_backward(
 
     if (R == 0 && keep_records) {
         cudaError_t e = cudaMemsetAsync(geom.acc16, 0, (size_t)P * 64, stream);
-        if (e != cudaSuccess) return gh_check_cuda(e, "memset(accumulation records)");
+        if (e != cudaSuccess) return gh_cuda_status("gh_backward", "memset(accumulation records)", e);
     }
     if (R == 0) {
         // nothing was rendered: every gradient is zero (P * floats-per-row each)
@@ -380,7 +361,7 @@ int gh_backward(
         for (auto& b : z)
             if (b.p) {
                 cudaError_t e = cudaMemsetAsync(b.p, 0, (size_t)P * b.n * sizeof(float), stream);
-                if (e != cudaSuccess) return gh_check_cuda(e, "memset(gradients)");
+                if (e != cudaSuccess) return gh_cuda_status("gh_backward", "memset(gradients)", e);
             }
     }
     if (R > 0 && det_buffer != nullptr) {
@@ -392,7 +373,7 @@ int gh_backward(
             uint32_t total = 0;
             cudaError_t e = cudaMemcpyAsync(&total, det.off + P, sizeof(total), cudaMemcpyDeviceToHost, stream);
             if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
-            if (e != cudaSuccess) return gh_check_cuda(e, "read back the row count");
+            if (e != cudaSuccess) return gh_cuda_status("gh_backward", "read back the row count", e);
             if (total != (uint32_t)R)
                 return gh_set_error(GH_E_INVALID_ARG, "gh_backward: the tile rectangles of radii do not add up to R");
         }
@@ -407,7 +388,7 @@ int gh_backward(
     } else if (R > 0) {
         GhStageTimer t(GH_ST_BLEND_BWD, stream);
         cudaError_t e = cudaMemsetAsync(geom.acc16, 0, (size_t)P * 64, stream);
-        if (e != cudaSuccess) return gh_check_cuda(e, "memset(accumulation records)");
+        if (e != cudaSuccess) return gh_cuda_status("gh_backward", "memset(accumulation records)", e);
         gh_launch_blend_backward(width, height, gx, gy, geom, img, bin, colors_precomp, background, dL_dpix, stream);
         g_launches += 1;
         if (conic_precomp != nullptr && !keep_records) {   // otherwise the geometry backward unpacks the records itself
@@ -416,7 +397,7 @@ int gh_backward(
             g_launches += 1;
         }
     }
-    GH_STAGE(stream, debug, "blend backward");
+    GH_STAGE("gh_backward", stream, debug, "blend backward");
     if (conic_precomp == nullptr && R > 0) {   // reference: geometry backward is a no-op when the conic was supplied
         GhStageTimer t(GH_ST_PREPROCESS_BWD, stream);
         gh_launch_preprocess_backward(P, means3D, radii, scales, scale_modifier, rotations, cov3D_precomp,
@@ -425,7 +406,7 @@ int gh_backward(
                                       dL_dmean3D, dL_dcov3D, dL_dscale, dL_drot, stream);
         g_launches += 1;
     }
-    GH_STAGE(stream, debug, "preprocess backward");
+    GH_STAGE("gh_backward", stream, debug, "preprocess backward");
     return GH_OK;
 }
 
@@ -434,12 +415,12 @@ int gh_mark_visible(int P, const float* means3D, const float* viewmatrix, const 
 {
     (void)projmatrix;
     cudaStream_t stream = (cudaStream_t)stream_;
-    g_err[0] = 0;
+    gh_clear_error();
     if (P < 0) return gh_set_error(GH_E_INVALID_ARG, "gh_mark_visible: negative P");
     if (P == 0) return GH_OK;
     if (!means3D || !viewmatrix || !present) return gh_set_error(GH_E_INVALID_ARG, "gh_mark_visible: missing pointer");
     gh_launch_mark_visible(P, means3D, viewmatrix, reinterpret_cast<bool*>(present), stream);
-    GH_STAGE(stream, 0, "mark visible");
+    GH_STAGE("gh_mark_visible", stream, 0, "mark visible");
     return GH_OK;
 }
 
@@ -451,7 +432,7 @@ int gh_debug_export(
     float* depths, float* means2D, float* conic_opacity, gh_stream_t stream_)
 {
     cudaStream_t stream = (cudaStream_t)stream_;
-    g_err[0] = 0;
+    gh_clear_error();
     if (P <= 0 || width <= 0 || height <= 0 || R < 0 || !geom_buffer || !img_buffer)
         return gh_set_error(GH_E_INVALID_ARG, "gh_debug_export: bad arguments");
     int gx, gy; const int T = gh_tile_grid(width, height, gx, gy);
@@ -469,8 +450,8 @@ int gh_debug_export(
     if (depths && e == cudaSuccess) e = cudaMemcpyAsync(depths, geom.depth, (size_t)P * 4, cudaMemcpyDeviceToDevice, stream);
     if ((means2D || conic_opacity) && e == cudaSuccess)
         gh_export_geom_kernel<<<(P + 255) / 256, 256, 0, stream>>>(P, geom.geo, means2D, conic_opacity);
-    if (e != cudaSuccess) return gh_check_cuda(e, "debug export");
-    GH_STAGE(stream, 0, "debug export");
+    if (e != cudaSuccess) return gh_cuda_status("gh_debug_export", "copy", e);
+    GH_STAGE("gh_debug_export", stream, 0, "debug export");
     return GH_OK;
 }
 

@@ -193,7 +193,7 @@ gh_tile_scan_kernel(int T, const uint32_t* __restrict__ tile_count, uint32_t* __
 // slots of the same few buckets: lanes that want the same tile in the same loop step are grouped
 // with match.any and their leader reserves all their slots with ONE atomic.
 // `capacity`: records the instance buffer holds.  The forward's first phase may launch emit before the host has read R
-// back (gh_forward_preprocess_ex): when R = ctrl->num_rendered exceeds the capacity, no thread writes anything and the
+// back (the binning buffer of gh_forward_preprocess): when R = ctrl->num_rendered exceeds the capacity, no thread writes anything and the
 // tile cursors stay as the scan left them, so the host can launch emit again into a buffer of the exact size.
 __global__ void __launch_bounds__(256)
 gh_emit_kernel(int P, const int* __restrict__ radii, const GhGeo* __restrict__ geo,

@@ -151,9 +151,7 @@ extern "C" int gh_densify_classify(int P, const float* grad_accum, const float* 
     if (P == 0) return GH_OK;
     gh_densify_classify_kernel<<<(P + 255) / 256, 256, 0, stream>>>(P, grad_accum, denom, log_scaling, opacity_logit,
                                                                    grad_threshold, dense_extent, min_opacity, ws_limit, flags);
-    gh_count_launches(1);
-    const cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? GH_OK : gh_set_error(GH_E_CUDA, cudaGetErrorString(e));
+    return gh_launch_status("gh_densify_classify", 1);
 }
 
 extern "C" int gh_densify_scatter(int P, int n_tensors, const float* const* src, const float* const* exp_avg,
@@ -191,7 +189,5 @@ extern "C" int gh_densify_scatter(int P, int n_tensors, const float* const* src,
         return gh_set_error(GH_E_INVALID_ARG, "gh_densify_scatter: xyz / scaling must have 3 and rotation 4 floats per Gaussian");
     gh_densify_scatter_kernel<<<(P + 127) / 128, 128, 0, stream>>>(P, T, flags, inclusive_prefix, n_keep, n_clone, n_split_kept,
                                                                   samples, n_split_all);
-    gh_count_launches(1);
-    const cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? GH_OK : gh_set_error(GH_E_CUDA, cudaGetErrorString(e));
+    return gh_launch_status("gh_densify_scatter", 1);
 }

@@ -553,8 +553,8 @@ extern "C" int gh_image_loss(int width, int height, const float* out_color, cons
     double* part_main = part_pointwise + 3 * (size_t)np.pb;
     float* dmaps = reinterpret_cast<float*>(part_main + np.mb);
     const size_t plane = (size_t)width * height;
-    if (cudaMemsetAsync(sums, 0, GH_LS_COUNT * sizeof(double), stream) != cudaSuccess)      // sums + tickets
-        return gh_set_error(GH_E_CUDA, "gh_image_loss: memset of the partial sums failed");
+    const cudaError_t e = cudaMemsetAsync(sums, 0, GH_LS_COUNT * sizeof(double), stream);     // sums + tickets
+    if (e != cudaSuccess) return gh_cuda_status("gh_image_loss", "memset(partial sums)", e);
     const int rb = np.rb, pb = np.pb;
     const dim3 grid((width + GH_LT - 1) / GH_LT, (height + GH_LT - 1) / GH_LT), block(256);
     if (deterministic) {
@@ -571,7 +571,5 @@ extern "C" int gh_image_loss(int width, int height, const float* out_color, cons
     }
     gh_loss_ssim_bwd_kernel<4><<<grid, block, 0, stream>>>(prm, out_color, gt_image, gt_mask, dmaps, dL_dout);
     gh_loss_finalize_kernel<<<rb, 256, 0, stream>>>(prm, sums, losses, dL_dout);
-    gh_count_launches(5);
-    const cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? GH_OK : gh_set_error(GH_E_CUDA, cudaGetErrorString(e));
+    return gh_launch_status("gh_image_loss", 5);
 }

@@ -56,7 +56,7 @@ void gh_launch_preprocess_backward(int P, const float* means3D, const int* radii
                                    float* dL_dmean3D, float* dL_dcov3D, float* dL_dscale, float* dL_drot,
                                    cudaStream_t stream);
 
-// The forward's first phase around its per-Gaussian kernel (gh_forward_preprocess[_ex], gh_project_forward_binned[_ex]):
+// The forward's first phase around its per-Gaussian kernel (gh_forward_preprocess, gh_project_forward_binned):
 // tile grid and its bound, workspace carving, ctrl + histogram memset, `bin(geom, img, gx, gy)` (launches the kernel on
 // `stream` and counts it), tile scan, read-back of R and the longest tile list.  `who` names the entry point in error
 // messages.  With a binning buffer of `bin_capacity` records (`radii` then names the radii the kernel writes), emit is
@@ -77,13 +77,20 @@ int gh_forward_phase1(const char* who, int P, int width, int height, char* geom_
     return gh_forward_phase1(who, P, width, height, geom_buffer, img_buffer, num_rendered, max_tile_len, debug, stream, emit,
                              [](const void* f, const GhGeomWS& g, const GhImgWS& i, int gx, int gy) { (*static_cast<const F*>(f))(g, i, gx, gy); }, &bin);
 }
-// argument checks of the optional binning buffer of the *_ex entry points (before any launch)
+// argument checks of the optional binning buffer of the first-phase entry points (before any launch)
 int gh_check_phase1_bin(const char* who, const GhPhase1Bin& emit);
 
 // per-thread error message behind gh_last_error(): every extern "C" entry point clears it on entry and
-// sets it before returning a GH_E_* code (defined in gh_api.cu)
+// sets it before returning a GH_E_* code (defined in gh_api.cu).  gh_set_error is its only writer (printf-style,
+// returns `code`).
 void gh_clear_error();
-int gh_set_error(int code, const char* msg);
+int gh_set_error(int code, const char* fmt, ...) __attribute__((format(printf, 2, 3)));
+// after `n` kernel launches: counts them (gh_count_launches) and returns GH_OK, or GH_E_CUDA with
+// "[CUDA ERROR] <who>: <cudaGetErrorString>" if a launch failed
+int gh_launch_status(const char* who, int n);
+// status of a CUDA runtime call (memset, attribute, event, host API): GH_OK, or GH_E_CUDA with
+// "[CUDA ERROR] <who>: <what>: <cudaGetErrorString>"
+int gh_cuda_status(const char* who, const char* what, cudaError_t e);
 
 // kernels launched outside gh_api.cu (optimizer, image losses) report themselves to gh_kernel_launch_count()
 void gh_count_launches(int n);

@@ -18,7 +18,6 @@
 #include "../../include/gh_rasterizer.h"
 
 #include <climits>
-#include <cstdio>
 
 namespace {
 
@@ -255,34 +254,12 @@ gh_knn_query_kernel(int P, int depth, const float4* __restrict__ pts, const floa
 
 int gh_knn_check(const char* who, long long P, const void* points, const void* workspace, size_t bytes)
 {
-    char msg[160];
-    if (P < 0 || P > INT_MAX) {
-        std::snprintf(msg, sizeof(msg), "%s: P must lie in [0, 2^31)", who);
-        return gh_set_error(GH_E_INVALID_ARG, msg);
-    }
-    if (P > 0 && (!points || !workspace)) {
-        std::snprintf(msg, sizeof(msg), "%s: missing points or workspace", who);
-        return gh_set_error(GH_E_INVALID_ARG, msg);
-    }
-    if (P > 0 && ((size_t)points & 3)) {
-        std::snprintf(msg, sizeof(msg), "%s: points must be 4-byte aligned", who);
-        return gh_set_error(GH_E_INVALID_ARG, msg);
-    }
-    if (P > 0 && bytes < GhKnnWS::bytes((size_t)P)) {
-        std::snprintf(msg, sizeof(msg), "%s: workspace smaller than gh_knn_workspace_size", who);
-        return gh_set_error(GH_E_INVALID_ARG, msg);
-    }
+    if (P < 0 || P > INT_MAX) return gh_set_error(GH_E_INVALID_ARG, "%s: P must lie in [0, 2^31)", who);
+    if (P > 0 && (!points || !workspace)) return gh_set_error(GH_E_INVALID_ARG, "%s: missing points or workspace", who);
+    if (P > 0 && ((size_t)points & 3)) return gh_set_error(GH_E_INVALID_ARG, "%s: points must be 4-byte aligned", who);
+    if (P > 0 && bytes < GhKnnWS::bytes((size_t)P))
+        return gh_set_error(GH_E_INVALID_ARG, "%s: workspace smaller than gh_knn_workspace_size", who);
     return GH_OK;
-}
-
-int gh_knn_status(int launches)
-{
-    gh_count_launches(launches);
-    const cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) return GH_OK;
-    char msg[256];
-    std::snprintf(msg, sizeof(msg), "[CUDA ERROR] knn: %s", cudaGetErrorString(e));
-    return gh_set_error(GH_E_CUDA, msg);
 }
 
 }  // namespace
@@ -306,12 +283,12 @@ extern "C" int gh_knn_morton(long long P, const float* points, long long* codes,
     if (!codes || ((size_t)codes & 7)) return gh_set_error(GH_E_INVALID_ARG, "gh_knn_morton: codes must be an 8-byte aligned int64 array");
     const GhKnnWS ws = GhKnnWS::carve((char*)workspace, (size_t)P);
     const cudaError_t e = cudaMemsetAsync(ws.box, 0, 6 * sizeof(unsigned int), stream);
-    if (e != cudaSuccess) return gh_set_error(GH_E_CUDA, "[CUDA ERROR] knn: memset(bounding box)");
+    if (e != cudaSuccess) return gh_cuda_status("gh_knn_morton", "memset(bounding box)", e);
     const int n = (int)P;
     const int blocks = (n + 255) / 256;
     gh_knn_bbox_kernel<<<min(blocks, 1024), 256, 0, stream>>>(n, points, ws.box);
     gh_knn_morton_kernel<<<blocks, 256, 0, stream>>>(n, points, ws.box, codes);
-    return gh_knn_status(2);
+    return gh_launch_status("gh_knn_morton", 2);
 }
 
 extern "C" int gh_knn_mean_dist3(long long P, const float* points, const long long* order, float* out, void* workspace,
@@ -337,5 +314,5 @@ extern "C" int gh_knn_mean_dist3(long long P, const float* points, const long lo
         row -= steps;
     }
     gh_knn_query_kernel<<<(n + 127) / 128, 128, 0, stream>>>(n, ws.depth, ws.pts, ws.nodes, out);
-    return gh_knn_status(launches + 1);
+    return gh_launch_status("gh_knn_mean_dist3", launches + 1);
 }

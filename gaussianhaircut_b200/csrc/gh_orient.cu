@@ -15,7 +15,6 @@
 #include "../../include/gh_rasterizer.h"
 
 #include <climits>
-#include <cstdio>
 
 namespace {
 
@@ -256,51 +255,27 @@ size_t gh_orient_smem_bytes(int K, int nf)
 
 int gh_orient_check_image(const char* who, int H, int W)
 {
-    char msg[160];
-    if (H <= 0 || W <= 0 || (long long)H * W >= (1ll << 31)) {
-        std::snprintf(msg, sizeof(msg), "%s: H and W must be positive with H*W < 2^31", who);
-        return gh_set_error(GH_E_INVALID_ARG, msg);
-    }
+    if (H <= 0 || W <= 0 || (long long)H * W >= (1ll << 31))
+        return gh_set_error(GH_E_INVALID_ARG, "%s: H and W must be positive with H*W < 2^31", who);
     return GH_OK;
 }
 
 int gh_orient_check_bank(const char* who, int N, int K, int nf)
 {
-    char msg[200];
-    if (K < 1 || K > GH_ORIENT_MAX_K || (K & 1) == 0) {
-        std::snprintf(msg, sizeof(msg), "%s: K must be odd and in [1, %d]", who, GH_ORIENT_MAX_K);
-        return gh_set_error(GH_E_INVALID_ARG, msg);
-    }
-    if (nf < 1 || nf > GH_ORIENT_MAX_FILTERS || N < nf || N > GH_ORIENT_MAX_N || N % nf != 0) {
-        std::snprintf(msg, sizeof(msg), "%s: need 1 <= num_filters <= %d and N a multiple of num_filters, N <= %d", who,
-                      GH_ORIENT_MAX_FILTERS, GH_ORIENT_MAX_N);
-        return gh_set_error(GH_E_INVALID_ARG, msg);
-    }
+    if (K < 1 || K > GH_ORIENT_MAX_K || (K & 1) == 0)
+        return gh_set_error(GH_E_INVALID_ARG, "%s: K must be odd and in [1, %d]", who, GH_ORIENT_MAX_K);
+    if (nf < 1 || nf > GH_ORIENT_MAX_FILTERS || N < nf || N > GH_ORIENT_MAX_N || N % nf != 0)
+        return gh_set_error(GH_E_INVALID_ARG, "%s: need 1 <= num_filters <= %d and N a multiple of num_filters, N <= %d", who,
+                            GH_ORIENT_MAX_FILTERS, GH_ORIENT_MAX_N);
     return GH_OK;
 }
 
 int gh_orient_check_ws(const char* who, const void* workspace, size_t bytes, size_t need)
 {
-    char msg[160];
-    if (!workspace || ((size_t)workspace & 255)) {
-        std::snprintf(msg, sizeof(msg), "%s: workspace must be a 256-byte aligned device pointer", who);
-        return gh_set_error(GH_E_INVALID_ARG, msg);
-    }
-    if (bytes < need) {
-        std::snprintf(msg, sizeof(msg), "%s: workspace smaller than gh_orient_workspace_size", who);
-        return gh_set_error(GH_E_INVALID_ARG, msg);
-    }
+    if (!workspace || ((size_t)workspace & 255))
+        return gh_set_error(GH_E_INVALID_ARG, "%s: workspace must be a 256-byte aligned device pointer", who);
+    if (bytes < need) return gh_set_error(GH_E_INVALID_ARG, "%s: workspace smaller than gh_orient_workspace_size", who);
     return GH_OK;
-}
-
-int gh_orient_status(int launches)
-{
-    gh_count_launches(launches);
-    const cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) return GH_OK;
-    char msg[256];
-    std::snprintf(msg, sizeof(msg), "[CUDA ERROR] orient: %s", cudaGetErrorString(e));
-    return gh_set_error(GH_E_CUDA, msg);
 }
 
 }  // namespace
@@ -337,7 +312,7 @@ extern "C" int gh_orient_dog(int H, int W, int C, const unsigned char* image, co
     gh_orient_gray_kernel<<<blocks, 256, 0, stream>>>(n, C, image, ws.gray);
     gh_orient_dog_axis0_kernel<<<blocks, 256, 0, stream>>>(H, W, ws.gray, w_low, r_low, w_high, r_high, ws.tlo, ws.thi);
     gh_orient_dog_axis1_kernel<<<blocks, 256, 0, stream>>>(H, W, ws.tlo, ws.thi, w_low, r_low, w_high, r_high, dog, ws.dog32);
-    return gh_orient_status(3);
+    return gh_launch_status("gh_orient_dog", 3);
 }
 
 extern "C" int gh_orient_gabor(int H, int W, const float* bank, int N, int K, int num_filters, const float* thetas,
@@ -358,10 +333,10 @@ extern "C" int gh_orient_gabor(int H, int W, const float* bank, int N, int K, in
     const int G = N / num_filters, nch = (num_filters + GH_OR_CHUNK - 1) / GH_OR_CHUNK;
     const size_t smem = gh_orient_smem_bytes(K, num_filters);
     const cudaError_t e = cudaFuncSetAttribute(gh_orient_gabor_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return gh_set_error(GH_E_CUDA, "[CUDA ERROR] orient: cudaFuncSetAttribute(shared memory)");
+    if (e != cudaSuccess) return gh_cuda_status("gh_orient_gabor", "cudaFuncSetAttribute(shared memory)", e);
     gh_orient_bank_kernel<<<G * nch, GH_OR_THREADS, 0, stream>>>(K, num_filters, G, nch, bank, ws.wbank, ws.sup);
     const long long tiles = (long long)((W + GH_OR_TILE - 1) / GH_OR_TILE) * ((H + GH_OR_TILE - 1) / GH_OR_TILE);
     gh_orient_gabor_kernel<<<(unsigned int)tiles, GH_OR_THREADS, smem, stream>>>(H, W, K, num_filters, G, nch, ws.dog32,
                                                                                ws.wbank, ws.sup, thetas, orients, var);
-    return gh_orient_status(2);
+    return gh_launch_status("gh_orient_gabor", 2);
 }

@@ -31,8 +31,6 @@
 #include "../../include/gh_rasterizer.h"
 #include "gh_project_math.h"
 
-#include <cstdio>
-
 namespace {
 
 #define GH_PJ_THREADS 128
@@ -269,24 +267,22 @@ gh_project_backward_kernel(GhProjArgs A, const unsigned char* __restrict__ mask,
 
 int gh_proj_check(GhProjArgs& A, const char* who, bool strand)
 {
-    char msg[160];
-    if (A.P <= 0 || A.W <= 0 || A.H <= 0) { snprintf(msg, sizeof msg, "%s: P, width, height must be positive", who); return gh_set_error(GH_E_INVALID_ARG, msg); }
+    if (A.P <= 0 || A.W <= 0 || A.H <= 0) return gh_set_error(GH_E_INVALID_ARG, "%s: P, width, height must be positive", who);
     if (strand) {
-        if (A.rotation) { snprintf(msg, sizeof msg, "%s: strand mode derives the rotation from dirs, rotation must be NULL", who); return gh_set_error(GH_E_INVALID_ARG, msg); }
-        if (!A.dirs) { snprintf(msg, sizeof msg, "%s: strand mode needs dirs (the segment vectors)", who); return gh_set_error(GH_E_INVALID_ARG, msg); }
-        if (!A.scaling) { snprintf(msg, sizeof msg, "%s: strand mode needs scaling = the strand thickness (one device float)", who); return gh_set_error(GH_E_INVALID_ARG, msg); }
-        if (A.scale_act != 0 || A.dir_mode != 1) { snprintf(msg, sizeof msg, "%s: strand mode needs scale activation 0 and direction mode 1", who); return gh_set_error(GH_E_INVALID_ARG, msg); }
+        if (A.rotation) return gh_set_error(GH_E_INVALID_ARG, "%s: strand mode derives the rotation from dirs, rotation must be NULL", who);
+        if (!A.dirs) return gh_set_error(GH_E_INVALID_ARG, "%s: strand mode needs dirs (the segment vectors)", who);
+        if (!A.scaling) return gh_set_error(GH_E_INVALID_ARG, "%s: strand mode needs scaling = the strand thickness (one device float)", who);
+        if (A.scale_act != 0 || A.dir_mode != 1) return gh_set_error(GH_E_INVALID_ARG, "%s: strand mode needs scale activation 0 and direction mode 1", who);
     }
-    if (!A.xyz || !A.scaling || (!strand && !A.rotation) || !A.f_dc || !A.V || !A.Pm || !A.campos) { snprintf(msg, sizeof msg, "%s: missing mandatory pointer", who); return gh_set_error(GH_E_INVALID_ARG, msg); }
-    if (A.sh_degree < 0 || A.sh_degree > 3) { snprintf(msg, sizeof msg, "%s: sh_degree must be 0..3", who); return gh_set_error(GH_E_INVALID_ARG, msg); }
-    if (A.sh_degree > 0 && !A.f_rest) { snprintf(msg, sizeof msg, "%s: features_rest required for sh_degree > 0", who); return gh_set_error(GH_E_INVALID_ARG, msg); }
-    if ((size_t)A.rotation & 15) { snprintf(msg, sizeof msg, "%s: rotation must be 16-byte aligned", who); return gh_set_error(GH_E_INVALID_ARG, msg); }
-    if (A.dir_mode == 1 && !A.dirs) { snprintf(msg, sizeof msg, "%s: dirs required for dir_mode 1", who); return gh_set_error(GH_E_INVALID_ARG, msg); }
-    if ((A.opacity_act < 2 && !A.opacity) || (A.label_act < 2 && !A.label) || (A.conf_act < 2 && !A.conf)) {
-        snprintf(msg, sizeof msg, "%s: opacity / label / orient_conf pointer missing for the chosen activation", who);
-        return gh_set_error(GH_E_INVALID_ARG, msg);
-    }
-    if (!(A.tanx > 0.f) || !(A.tany > 0.f)) { snprintf(msg, sizeof msg, "%s: tan_fov must be positive", who); return gh_set_error(GH_E_INVALID_ARG, msg); }
+    if (!A.xyz || !A.scaling || (!strand && !A.rotation) || !A.f_dc || !A.V || !A.Pm || !A.campos)
+        return gh_set_error(GH_E_INVALID_ARG, "%s: missing mandatory pointer", who);
+    if (A.sh_degree < 0 || A.sh_degree > 3) return gh_set_error(GH_E_INVALID_ARG, "%s: sh_degree must be 0..3", who);
+    if (A.sh_degree > 0 && !A.f_rest) return gh_set_error(GH_E_INVALID_ARG, "%s: features_rest required for sh_degree > 0", who);
+    if ((size_t)A.rotation & 15) return gh_set_error(GH_E_INVALID_ARG, "%s: rotation must be 16-byte aligned", who);
+    if (A.dir_mode == 1 && !A.dirs) return gh_set_error(GH_E_INVALID_ARG, "%s: dirs required for dir_mode 1", who);
+    if ((A.opacity_act < 2 && !A.opacity) || (A.label_act < 2 && !A.label) || (A.conf_act < 2 && !A.conf))
+        return gh_set_error(GH_E_INVALID_ARG, "%s: opacity / label / orient_conf pointer missing for the chosen activation", who);
+    if (!(A.tanx > 0.f) || !(A.tany > 0.f)) return gh_set_error(GH_E_INVALID_ARG, "%s: tan_fov must be positive", who);
     return GH_OK;
 }
 
@@ -340,14 +336,12 @@ extern "C" int gh_project_forward(
     auto kernel = strand ? gh_project_forward_kernel<false, true> : gh_project_forward_kernel<false, false>;
     kernel<<<(P + GH_PJ_THREADS - 1) / GH_PJ_THREADS, GH_PJ_THREADS, 0, stream>>>(
         A, means2D, colors, opacities, conic, cov3D, visible, nullptr, nullptr, nullptr, nullptr, 0, 0);
-    gh_count_launches(1);
-    const cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? GH_OK : gh_set_error(GH_E_CUDA, cudaGetErrorString(e));
+    return gh_launch_status("gh_project_forward", 1);
 }
 
-// gh_project_forward + the rasterizer's first phase (gh_forward_phase1, as in gh_forward_preprocess_ex) in one pass over
-// the Gaussians; continue with gh_forward_render_ex.
-extern "C" int gh_project_forward_binned_ex(
+// gh_project_forward + the rasterizer's first phase (gh_forward_phase1, as in gh_forward_preprocess) in one pass over
+// the Gaussians; continue with gh_forward_render.
+extern "C" int gh_project_forward_binned(
     int P, int width, int height,
     const float* xyz, const float* scaling, const float* rotation, const float* dirs,
     const float* features_dc, const float* features_rest,
@@ -378,23 +372,6 @@ extern "C" int gh_project_forward_binned_ex(
             A, means2D, colors, opacities, conic, cov3D, visible, radii, geom.geo, geom.depth, img.tile_count, gx, gy);
         gh_count_launches(1);
     });
-}
-
-extern "C" int gh_project_forward_binned(
-    int P, int width, int height,
-    const float* xyz, const float* scaling, const float* rotation, const float* dirs,
-    const float* features_dc, const float* features_rest,
-    const float* opacity, const float* label, const float* orient_conf,
-    const float* viewmatrix, const float* projmatrix, const float* campos,
-    float tan_fovx, float tan_fovy, float scale_modifier, int sh_degree, unsigned int flags, float det_eps,
-    float* means2D, float* colors, float* opacities, float* conic, float* cov3D, unsigned char* visible,
-    int* radii, char* geom_buffer, char* img_buffer, int* num_rendered, int* max_tile_len,
-    gh_stream_t stream_)
-{
-    return gh_project_forward_binned_ex(P, width, height, xyz, scaling, rotation, dirs, features_dc, features_rest, opacity,
-                                        label, orient_conf, viewmatrix, projmatrix, campos, tan_fovx, tan_fovy, scale_modifier,
-                                        sh_degree, flags, det_eps, means2D, colors, opacities, conic, cov3D, visible, radii,
-                                        geom_buffer, img_buffer, nullptr, 0, num_rendered, max_tile_len, nullptr, stream_);
 }
 
 extern "C" int gh_project_backward(
@@ -436,15 +413,13 @@ extern "C" int gh_project_backward(
     float* partial = workspace ? reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256) : nullptr;
     if (d_camera != nullptr) {
         // the ticket word is reset by the kernel's last CTA; zero it here for the very first use of a workspace
-        if (cudaMemsetAsync(ticket, 0, sizeof(unsigned int), stream) != cudaSuccess)
-            return gh_set_error(GH_E_CUDA, "gh_project_backward: memset(ticket) failed");
+        const cudaError_t e = cudaMemsetAsync(ticket, 0, sizeof(unsigned int), stream);
+        if (e != cudaSuccess) return gh_cuda_status("gh_project_backward", "memset(ticket)", e);
     }
     auto kernel = strand ? gh_project_backward_kernel<true> : gh_project_backward_kernel<false>;
     kernel<<<(P + GH_PJ_THREADS - 1) / GH_PJ_THREADS, GH_PJ_THREADS, 0, stream>>>(
         A, visible, acc16, dL_dmeans2D, dL_dconic, dL_dcolors, dL_dopacity,
         d_xyz, d_scaling, d_rotation, d_dirs, d_features_dc, d_features_rest, d_opacity, d_label, d_orient_conf,
         d_means2D, partial, ticket, d_camera, nan_flag);
-    gh_count_launches(1);
-    const cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? GH_OK : gh_set_error(GH_E_CUDA, cudaGetErrorString(e));
+    return gh_launch_status("gh_project_backward", 1);
 }

@@ -14,8 +14,6 @@
 #include "gh_kernels.h"
 #include "../../include/gh_rasterizer.h"
 
-#include <cstdio>
-
 namespace {
 
 #define GH_ST_THREADS 128
@@ -87,9 +85,8 @@ gh_strand_backward_kernel(int S, int L, const float* __restrict__ d_xyz, float* 
 
 int gh_strand_check(int S, int L, const char* who)
 {
-    char msg[160];
-    if (S <= 0 || L <= 0) { snprintf(msg, sizeof msg, "%s: S and L must be positive", who); return gh_set_error(GH_E_INVALID_ARG, msg); }
-    if ((unsigned long long)S * L * 3 > 0x7fffffffull) { snprintf(msg, sizeof msg, "%s: 3 * S * L must stay below 2^31", who); return gh_set_error(GH_E_INVALID_ARG, msg); }
+    if (S <= 0 || L <= 0) return gh_set_error(GH_E_INVALID_ARG, "%s: S and L must be positive", who);
+    if ((unsigned long long)S * L * 3 > 0x7fffffffull) return gh_set_error(GH_E_INVALID_ARG, "%s: 3 * S * L must stay below 2^31", who);
     return GH_OK;
 }
 
@@ -103,9 +100,7 @@ extern "C" int gh_strand_midpoints(int S, int L, const float* origins, const flo
     if (rc != GH_OK) return rc;
     if (!origins || !dirs || !xyz) return gh_set_error(GH_E_INVALID_ARG, "gh_strand_midpoints: missing pointer");
     gh_strand_midpoints_kernel<<<(3 * S + GH_ST_THREADS - 1) / GH_ST_THREADS, GH_ST_THREADS, 0, stream>>>(S, L, origins, dirs, xyz);
-    gh_count_launches(1);
-    const cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? GH_OK : gh_set_error(GH_E_CUDA, cudaGetErrorString(e));
+    return gh_launch_status("gh_strand_midpoints", 1);
 }
 
 extern "C" int gh_strand_backward(int S, int L, const float* d_xyz, float* d_dirs, unsigned int* nan_flag, gh_stream_t stream_)
@@ -116,7 +111,5 @@ extern "C" int gh_strand_backward(int S, int L, const float* d_xyz, float* d_dir
     if (rc != GH_OK) return rc;
     if (!d_xyz || !d_dirs) return gh_set_error(GH_E_INVALID_ARG, "gh_strand_backward: missing pointer");
     gh_strand_backward_kernel<<<(S + GH_ST_WARPS - 1) / GH_ST_WARPS, GH_ST_THREADS, 0, stream>>>(S, L, d_xyz, d_dirs, nan_flag);
-    gh_count_launches(1);
-    const cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? GH_OK : gh_set_error(GH_E_CUDA, cudaGetErrorString(e));
+    return gh_launch_status("gh_strand_backward", 1);
 }

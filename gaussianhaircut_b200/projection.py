@@ -139,7 +139,7 @@ def project_forward_binned(pi: ProjectionInputs, means2D_out: Optional[torch.Ten
     buf, capacity = _C.binning_hint(key) if binning else (None, 0)
     n_rendered, max_len, emitted = C.c_int(0), C.c_int(0), C.c_int(0)
     with torch.cuda.device(dev):
-        _capi.check(lib.gh_project_forward_binned_ex(
+        _capi.check(lib.gh_project_forward_binned(
             *_common_args(pi), _ptr(out["means2D"]), _ptr(out["colors"]), _ptr(out["opacity"]), _ptr(out["conic"]), None,
             _ptr(out["visible"]), _ptr(radii), _ptr(geom), _ptr(img), _ptr(buf), capacity,
             C.byref(n_rendered), C.byref(max_len), C.byref(emitted), _stream(dev)))

@@ -37,9 +37,11 @@
  * at rasterizer_impl.cu:285):
  *   1. gh_forward_workspace_sizes(P, W, H, &geom_bytes, &img_bytes); allocate both.
  *   2. gh_forward_preprocess(...): runs preprocess + per-tile histogram + scan, then copies the
- *      instance count R (= the reference's num_rendered) to the host and returns it.
+ *      instance count R (= the reference's num_rendered) to the host and returns it.  Optionally it is
+ *      handed a binning buffer sized from a guess of R; if R fits, it also runs the bucket scatter
+ *      (*emitted = 1) and step 3 is skipped.
  *   3. gh_binning_workspace_size(R, &bytes); allocate.
- *   4. gh_forward_render(...): bucket scatter, per-tile sort, alpha compositing.
+ *   4. gh_forward_render(...): bucket scatter (unless emitted), per-tile sort, alpha compositing.
  * The three workspaces must be kept for gh_backward (the reference keeps its three byte tensors on
  * the autograd ctx, __init__.py:102).
  */
@@ -99,31 +101,14 @@ int gh_binning_workspace_size(long long R, size_t* binning_bytes);
  * taken from it.  means2D_precomp is never read (reference forward.cu:201-210).
  * Writes radii[P].  On return *num_rendered = R and *max_tile_len = longest per-tile list
  * (host values; the call synchronises `stream`).
+ * Optional binning buffer: given binning_buffer of gh_binning_workspace_size(binning_capacity) bytes, the bucket
+ * scatter (emit) is enqueued right behind the read-back of R, so it runs while the host waits and prepares phase 2.
+ * *emitted = 1 if R <= binning_capacity: the buffer then holds the binned instances (pass it, with emitted = 1, to
+ * gh_forward_render).  *emitted = 0 otherwise: nothing was written; size a buffer for R and call gh_forward_render
+ * with emitted = 0.  binning_buffer = NULL, binning_capacity = 0 (emitted may then be NULL) runs no scatter here.
+ * binning_capacity must lie in [0, 2^32); `emitted` is required with a buffer.
  */
 int gh_forward_preprocess(
-    int P, int D, int M,
-    int width, int height,
-    const float* means3D, const float* means2D_precomp, const float* shs,
-    const float* colors_precomp, const float* opacities,
-    const float* scales, float scale_modifier, const float* rotations,
-    const float* cov3D_precomp, const float* conic_precomp,
-    const float* viewmatrix, const float* projmatrix, const float* cam_pos,
-    float tan_fovx, float tan_fovy, int prefiltered,
-    int* radii,
-    char* geom_buffer, char* img_buffer,
-    int* num_rendered, int* max_tile_len,
-    int debug, gh_stream_t stream);
-
-/*
- * gh_forward_preprocess that may also bin: given a binning buffer of gh_binning_workspace_size(binning_capacity) bytes,
- * the bucket scatter (emit) is enqueued right behind the read-back of R, so it runs while the host waits and prepares
- * phase 2.  *emitted = 1 if R <= binning_capacity: the buffer then holds the binned instances (pass it, with
- * emitted = 1, to gh_forward_render_ex).  *emitted = 0 otherwise: nothing was written; size the buffer for R and call
- * gh_forward_render_ex with emitted = 0, exactly as after gh_forward_preprocess.  binning_buffer = NULL,
- * binning_capacity = 0 is gh_forward_preprocess.  binning_capacity must lie in [0, 2^32); `emitted` is required with a
- * buffer.
- */
-int gh_forward_preprocess_ex(
     int P, int D, int M,
     int width, int height,
     const float* means3D, const float* means2D_precomp, const float* shs,
@@ -141,18 +126,10 @@ int gh_forward_preprocess_ex(
 /*
  * Phase 2 of Rasterizer::forward: binning + per-tile sort + front-to-back blend.
  * out_color is (C, H, W) channel-major, fully overwritten (background included).
+ * emitted = 1 skips the bucket scatter that the first phase already ran into binning_buffer (gh_forward_preprocess /
+ * gh_project_forward_binned reported *emitted = 1 for this buffer); emitted = 0 runs it here.
  */
 int gh_forward_render(
-    int P, int width, int height,
-    const float* background, const float* colors_precomp,
-    const int* radii,
-    char* geom_buffer, char* binning_buffer, char* img_buffer,
-    int num_rendered, int max_tile_len,
-    float* out_color,
-    int debug, gh_stream_t stream);
-/* gh_forward_render; emitted = 1 skips the bucket scatter that the first phase already ran into binning_buffer
- * (gh_forward_preprocess_ex / gh_project_forward_binned_ex reported *emitted = 1 for this buffer). */
-int gh_forward_render_ex(
     int P, int width, int height,
     const float* background, const float* colors_precomp,
     const int* radii,
@@ -336,19 +313,9 @@ int gh_project_forward(
  * outputs of gh_project_forward it fills `radii` and the geometry / image workspaces exactly as gh_forward_preprocess
  * would when handed (xyz, conic, opacities) with prefiltered = 0 -- same device code, bit-identical radii, state
  * records and keys -- runs the tile scan and returns num_rendered / max_tile_len after the same 16-byte read-back.
- * Continue with gh_binning_workspace_size + gh_forward_render.  Workspaces: gh_forward_workspace_sizes. */
+ * binning_buffer, binning_capacity, emitted: the optional binning buffer of gh_forward_preprocess (same contract).
+ * Continue with gh_forward_render.  Workspaces: gh_forward_workspace_sizes. */
 int gh_project_forward_binned(
-    int P, int width, int height,
-    const float* xyz, const float* scaling, const float* rotation, const float* dirs,
-    const float* features_dc, const float* features_rest,
-    const float* opacity, const float* label, const float* orient_conf,
-    const float* viewmatrix, const float* projmatrix, const float* campos,
-    float tan_fovx, float tan_fovy, float scale_modifier, int sh_degree, unsigned int flags, float det_eps,
-    float* means2D, float* colors, float* opacities, float* conic, float* cov3D, unsigned char* visible,
-    int* radii, char* geom_buffer, char* img_buffer, int* num_rendered, int* max_tile_len,
-    gh_stream_t stream);
-/* gh_project_forward_binned with the optional binning buffer of gh_forward_preprocess_ex (same contract). */
-int gh_project_forward_binned_ex(
     int P, int width, int height,
     const float* xyz, const float* scaling, const float* rotation, const float* dirs,
     const float* features_dc, const float* features_rest,

@@ -1,11 +1,15 @@
-"""CPU tests of the first phase's optional binning buffer (gh_forward_preprocess_ex, gh_project_forward_binned_ex,
-gh_forward_render_ex) and of the capacity hint that sizes it (_C.binning_capacity): the ABI surface, and the refusal of
+"""CPU tests of the first phase's optional binning buffer (gh_forward_preprocess, gh_project_forward_binned,
+gh_forward_render) and of the capacity hint that sizes it (_C.binning_capacity): the ABI surface, and the refusal of
 bad buffer arguments before anything is launched."""
 import ctypes as C
+import os
+import re
 
 import pytest
 
 import _util  # noqa: F401  (puts the repository root on sys.path)
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.fixture(scope="module")
@@ -14,40 +18,50 @@ def lib():
     return _capi.load()
 
 
+def _header_params(name):
+    """Parameter names of `name` as declared in include/gh_rasterizer.h."""
+    src = open(os.path.join(ROOT, "include", "gh_rasterizer.h")).read()
+    decl = re.search(rf"\bint {name}\((.*?)\);", src, flags=re.S).group(1)
+    return [p.split()[-1].lstrip("*") for p in decl.split(",")]
+
+
 def test_abi_surface(lib):
     from gaussianhaircut_b200 import _capi
-    # additive: the existing entry points keep their signatures, so the ABI version is unchanged
-    assert lib.gh_abi_version() == _capi.ABI_VERSION == 4
+    # ABI 5: one entry point per forward phase; the optional binning buffer is part of each signature
+    assert lib.gh_abi_version() == _capi.ABI_VERSION == 5
     sig = _capi.SIGNATURES
-    pre, pre_ex = sig["gh_forward_preprocess"][1], sig["gh_forward_preprocess_ex"][1]
-    assert len(pre_ex) == len(pre) + 3
-    assert pre_ex[24:26] == [C.c_void_p, C.c_longlong]                   # binning_buffer, binning_capacity
-    ren, ren_ex = sig["gh_forward_render"][1], sig["gh_forward_render_ex"][1]
-    assert len(ren_ex) == len(ren) + 1 and ren_ex[11] is C.c_int          # emitted
-    pb, pb_ex = sig["gh_project_forward_binned"][1], sig["gh_project_forward_binned_ex"][1]
-    assert len(pb_ex) == len(pb) + 3 and pb_ex[30:32] == [C.c_void_p, C.c_longlong]
+    for name in ("gh_forward_preprocess_ex", "gh_forward_render_ex", "gh_project_forward_binned_ex"):
+        assert name not in sig and not hasattr(lib, name), name
+    for name, at in (("gh_forward_preprocess", 24), ("gh_project_forward_binned", 30)):
+        params, args = _header_params(name), sig[name][1]
+        assert len(params) == len(args), name
+        assert params[at:at + 2] == ["binning_buffer", "binning_capacity"], name
+        assert args[at:at + 2] == [C.c_void_p, C.c_longlong], name
+        assert params.index("emitted") == params.index("max_tile_len") + 1 and args[params.index("emitted")] == C.POINTER(C.c_int)
+    params, args = _header_params("gh_forward_render"), sig["gh_forward_render"][1]
+    assert len(params) == len(args) and params[11] == "emitted" and args[11] is C.c_int
 
 
-def _preprocess_ex(lib, buf, cap, emitted=True):
+def _preprocess(lib, buf, cap, emitted=True):
     fake = C.c_void_p(0x1000)
     n, m, e = C.c_int(), C.c_int(), C.c_int(7)
-    rc = lib.gh_forward_preprocess_ex(10, 3, 0, 64, 64, fake, None, None, fake, fake, fake, 1.0, fake, None, None,
-                                      fake, fake, fake, 0.5, 0.5, 0, fake, fake, fake, buf, cap,
-                                      C.byref(n), C.byref(m), C.byref(e) if emitted else None, 0, None)
+    rc = lib.gh_forward_preprocess(10, 3, 0, 64, 64, fake, None, None, fake, fake, fake, 1.0, fake, None, None,
+                                   fake, fake, fake, 0.5, 0.5, 0, fake, fake, fake, buf, cap,
+                                   C.byref(n), C.byref(m), C.byref(e) if emitted else None, 0, None)
     return rc
 
 
-def _project_binned_ex(lib, buf, cap, emitted=True):
+def _project_binned(lib, buf, cap, emitted=True):
     from gaussianhaircut_b200 import projection as pj
     fake = C.c_void_p(4096)
     common = (128, 64, 48, fake, fake, fake, fake, fake, fake, None, None, fake, fake, fake, fake,
               0.5, 0.5, 1.0, 3, pj.encode_flags(pj.HAIR_MODEL), 1e-7)
     n, m, e = C.c_int(), C.c_int(), C.c_int(7)
-    return lib.gh_project_forward_binned_ex(*common, fake, fake, fake, fake, None, fake, fake, fake, fake, buf, cap,
-                                            C.byref(n), C.byref(m), C.byref(e) if emitted else None, None)
+    return lib.gh_project_forward_binned(*common, fake, fake, fake, fake, None, fake, fake, fake, fake, buf, cap,
+                                         C.byref(n), C.byref(m), C.byref(e) if emitted else None, None)
 
 
-@pytest.mark.parametrize("entry", [_preprocess_ex, _project_binned_ex])
+@pytest.mark.parametrize("entry", [_preprocess, _project_binned])
 def test_bad_binning_arguments_are_refused_before_any_launch(lib, entry):
     from gaussianhaircut_b200 import _capi
     launches0 = lib.gh_kernel_launch_count()
@@ -62,22 +76,6 @@ def test_bad_binning_arguments_are_refused_before_any_launch(lib, entry):
         assert entry(lib, b, cap, emitted) == _capi.GH_E_INVALID_ARG, (b, cap, emitted)
         assert msg in lib.gh_last_error().decode(), (msg, lib.gh_last_error())
     assert lib.gh_kernel_launch_count() == launches0
-
-
-def test_ex_entry_points_keep_the_existing_checks(lib):
-    """The _ex entry points run every check of the entry point they extend, first."""
-    from gaussianhaircut_b200 import _capi
-    fake = C.c_void_p(0x1000)
-    n, m, e = C.c_int(), C.c_int(), C.c_int()
-    rc = lib.gh_forward_preprocess_ex(10, 3, 16, 64, 64, fake, None, fake, None, fake, fake, 1.0, fake, None, None,
-                                      fake, fake, fake, 0.5, 0.5, 0, fake, fake, fake, fake, 100,
-                                      C.byref(n), C.byref(m), C.byref(e), 0, None)
-    assert rc == _capi.GH_E_NO_COLORS
-    rc = lib.gh_forward_preprocess_ex(10, 3, 0, 40000, 40000, fake, None, None, fake, fake, fake, 1.0, fake, None,
-                                      None, fake, fake, fake, 0.5, 0.5, 0, fake, fake, fake, fake, 100,
-                                      C.byref(n), C.byref(m), C.byref(e), 0, None)
-    assert rc == _capi.GH_E_INVALID_ARG and b"image too large" in lib.gh_last_error()
-    assert lib.gh_forward_render_ex(0, 64, 64, fake, fake, fake, fake, fake, fake, 0, 0, 1, fake, 0, None) == _capi.GH_E_INVALID_ARG
 
 
 def test_capacity_hint():

@@ -161,7 +161,7 @@ def _forward_with_capacity(kw, s, capacity):
         _capi.check(lib.gh_binning_workspace_size(capacity, C.byref(nb)))
         buf = torch.full((nb.value,), 0xAB, dtype=torch.uint8, device=DEV)
     n, m, emitted = C.c_int(), C.c_int(), C.c_int(-1)
-    _capi.check(lib.gh_forward_preprocess_ex(
+    _capi.check(lib.gh_forward_preprocess(
         P, 3, 0, W, H, _ptr(kw["means3D"]), None, None, _ptr(kw["colors_precomp"]), _ptr(kw["opacities"]),
         _ptr(kw["scales"]), 1.0, _ptr(kw["rotations"]), None, None, _ptr(s["viewmatrix"]), _ptr(s["projmatrix"]),
         _ptr(s["campos"]), s["tanfovx"], s["tanfovy"], 0, _ptr(radii), _ptr(geom), _ptr(img), _ptr(buf),

@@ -60,31 +60,53 @@ def test_workspace_size_queries(lib):
     assert lib.gh_binning_workspace_size(-5, C.byref(b)) == 1
 
 
+def test_size_queries_clear_the_last_error(lib):
+    """Every entry point clears the calling thread's message on entry, the workspace size queries included: a
+    successful query after a failed call leaves gh_last_error() empty."""
+    from gaussianhaircut_b200 import _capi
+    g, i = C.c_size_t(), C.c_size_t()
+    queries = (lambda: lib.gh_forward_workspace_sizes(10, 64, 64, C.byref(g), C.byref(i)),
+               lambda: lib.gh_binning_workspace_size(100, C.byref(g)),
+               lambda: lib.gh_backward_det_workspace_size(10, 100, C.byref(g)))
+    for query in queries:
+        assert lib.gh_forward_workspace_sizes(-1, 10, 10, C.byref(g), C.byref(i)) == _capi.GH_E_INVALID_ARG
+        assert lib.gh_last_error() != b""
+        assert query() == _capi.GH_OK and lib.gh_last_error() == b""
+
+
 def test_argument_validation_without_gpu(lib):
     """Argument checks run before any CUDA call, so they are testable on the CPU box."""
     from gaussianhaircut_b200 import _capi
     launches0 = lib.gh_kernel_launch_count()      # (GPU tests earlier in the same process count too)
-    n, m = C.c_int(), C.c_int()
+    n, m, e = C.c_int(), C.c_int(), C.c_int()
     fake = C.c_void_p(0x1000)
-    # no colours: the reference throws "For non-RGB, provide precomputed Gaussian colors!"
-    rc = lib.gh_forward_preprocess(10, 3, 16, 64, 64, fake, None, fake, None, fake, fake, 1.0, fake, None, None,
-                                   fake, fake, fake, 0.5, 0.5, 0, fake, fake, fake, C.byref(n), C.byref(m), 0, None)
-    assert rc == _capi.GH_E_NO_COLORS and b"provide precomputed Gaussian colors" in lib.gh_last_error()
+    # without and with the optional binning buffer: its checks come after the existing ones
+    for buf, cap, emitted in ((None, 0, None), (fake, 100, C.byref(e))):
+        # no colours: the reference throws "For non-RGB, provide precomputed Gaussian colors!"
+        rc = lib.gh_forward_preprocess(10, 3, 16, 64, 64, fake, None, fake, None, fake, fake, 1.0, fake, None, None,
+                                       fake, fake, fake, 0.5, 0.5, 0, fake, fake, fake, buf, cap,
+                                       C.byref(n), C.byref(m), emitted, 0, None)
+        assert rc == _capi.GH_E_NO_COLORS and b"provide precomputed Gaussian colors" in lib.gh_last_error()
+        # an image whose tile grid leaves the exactness range of the tile enumeration (gx * gx * gy < 2^32) is refused
+        rc = lib.gh_forward_preprocess(10, 3, 0, 40000, 40000, fake, None, None, fake, fake, fake, 1.0, C.c_void_p(0x1000),
+                                       None, None, fake, fake, fake, 0.5, 0.5, 0, fake, fake, fake, buf, cap,
+                                       C.byref(n), C.byref(m), emitted, 0, None)
+        assert rc == _capi.GH_E_INVALID_ARG and b"image too large" in lib.gh_last_error()
     # neither scale/rotation nor cov3D nor conic
     rc = lib.gh_forward_preprocess(10, 3, 0, 64, 64, fake, None, None, fake, fake, None, 1.0, None, None, None,
-                                   fake, fake, fake, 0.5, 0.5, 0, fake, fake, fake, C.byref(n), C.byref(m), 0, None)
+                                   fake, fake, fake, 0.5, 0.5, 0, fake, fake, fake, None, 0, C.byref(n), C.byref(m), None, 0, None)
     assert rc == _capi.GH_E_INVALID_ARG and b"scale/rotation pair" in lib.gh_last_error()
     # misaligned rotations
     rc = lib.gh_forward_preprocess(10, 3, 0, 64, 64, fake, None, None, fake, fake, fake, 1.0, C.c_void_p(0x1004), None,
-                                   None, fake, fake, fake, 0.5, 0.5, 0, fake, fake, fake, C.byref(n), C.byref(m), 0, None)
+                                   None, fake, fake, fake, 0.5, 0.5, 0, fake, fake, fake, None, 0, C.byref(n), C.byref(m), None,
+                                   0, None)
     assert rc == _capi.GH_E_INVALID_ARG and b"16-byte" in lib.gh_last_error()
     with pytest.raises(_capi.GhError) as ei:
         _capi.check(rc)
     assert ei.value.code == _capi.GH_E_INVALID_ARG
-    # an image whose tile grid leaves the exactness range of the tile enumeration (gx * gx * gy < 2^32) is refused
-    rc = lib.gh_forward_preprocess(10, 3, 0, 40000, 40000, fake, None, None, fake, fake, fake, 1.0, C.c_void_p(0x1000), None,
-                                   None, fake, fake, fake, 0.5, 0.5, 0, fake, fake, fake, C.byref(n), C.byref(m), 0, None)
-    assert rc == _capi.GH_E_INVALID_ARG and b"image too large" in lib.gh_last_error()
+    # the second phase checks its sizes before anything else, also when the first phase emitted (emitted = 1)
+    assert lib.gh_forward_render(0, 64, 64, fake, fake, fake, fake, fake, fake, 0, 0, 1, fake, 0, None) == _capi.GH_E_INVALID_ARG
+    assert b"gh_forward_render: bad sizes" in lib.gh_last_error()
     assert lib.gh_mark_visible(0, None, None, None, None, None) == 0
     assert lib.gh_kernel_launch_count() == launches0      # nothing was launched by any of the above
 

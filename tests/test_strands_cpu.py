@@ -193,7 +193,8 @@ def _proj_call(lib, which, flags, rotation=True, dirs=True, scaling=True, d_scal
         return lib.gh_project_forward(*common, fake, fake, fake, fake, None, fake, None)
     if which == "binned":
         n, m = C.c_int(0), C.c_int(0)
-        return lib.gh_project_forward_binned(*common, fake, fake, fake, fake, None, fake, fake, fake, fake, C.byref(n), C.byref(m), None)
+        return lib.gh_project_forward_binned(*common, fake, fake, fake, fake, None, fake, fake, fake, fake, None, 0,
+                                             C.byref(n), C.byref(m), None, None)
     return lib.gh_project_backward(*common, fake, None, fake, fake, fake, fake, fake, nz(d_scaling), nz(d_rotation), nz(d_dirs),
                                    fake, fake, None, None, fake, None, None, None, None, None)
 

@@ -117,11 +117,22 @@ _BIN_KEYS = 64          # shapes remembered (a model that grows changes P): the 
 _BIN_R: dict = {}
 
 
+def capacity_for(r_max: int) -> int:
+    """The capacity policy of the binning buffer: the largest R seen plus a quarter and 256 records."""
+    return r_max + r_max // 4 + 256
+
+
 def binning_capacity(key) -> int:
     """Records the first phase's binning buffer is sized for, for a forward keyed `key` = (device index, P, W, H): the
     largest of the last R seen for it plus a quarter (and 256 records), 0 when none has been seen."""
     seen = _BIN_R.get(key)
-    return max(seen) + max(seen) // 4 + 256 if seen else 0
+    return capacity_for(max(seen)) if seen else 0
+
+
+def last_num_rendered(key) -> int:
+    """R of the last forward keyed `key` (see binning_capacity), 0 when none has been seen."""
+    seen = _BIN_R.get(key)
+    return seen[-1] if seen else 0
 
 
 def binning_hint(key):
@@ -196,6 +207,52 @@ def _render(background, colors, radii, geomBuffer, imgBuffer, num_rendered, max_
         int(num_rendered), int(max_tile_len), int(binned is not None), _ptr(out_color), int(bool(debug)),
         stream if stream is not None else _stream(device)))
     return binningBuffer
+
+
+# ------------------------------------------------------------------------------------------------ capturable forward
+# The wrappers of the capturable entry points (include/gh_rasterizer.h): no host read of R, no `.item()`, no capacity
+# history -- the caller owns the binning buffer of `capacity` records and the device status word.
+def binning_workspace(capacity: int, device: torch.device) -> torch.Tensor:
+    """A binning buffer of `capacity` records (gh_binning_workspace_size)."""
+    nbytes = C.c_size_t()
+    _capi.check(_capi.load().gh_binning_workspace_size(int(capacity), C.byref(nbytes)))
+    return torch.empty(nbytes.value, dtype=torch.uint8, device=device)
+
+
+def forward_render_capturable(background, colors, geomBuffer, binningBuffer, imgBuffer, capacity: int,
+                              image_height: int, image_width: int) -> torch.Tensor:
+    """gh_forward_render_capturable on the workspaces of projection.project_forward_binned_capturable -> out_color
+    (C,H,W)."""
+    device = colors.device
+    with torch.cuda.device(device):
+        out_color = torch.empty((NUM_CHANNELS, int(image_height), int(image_width)), dtype=torch.float32, device=device)
+        colors = _prep(colors, "colors", device, align=8)
+        _capi.check(_capi.load().gh_forward_render_capturable(
+            int(colors.shape[0]), int(image_width), int(image_height), int(capacity),
+            _ptr(_prep(background, "background", device)), _ptr(colors), _ptr(geomBuffer), _ptr(binningBuffer),
+            _ptr(imgBuffer), _ptr(out_color), 0, _stream(device)))
+    return out_color
+
+
+def backward_records_capturable(background, colors, radii, geomBuffer, binningBuffer, imgBuffer, capacity: int,
+                                dL_dout_color) -> None:
+    """gh_backward_capturable: the blend backward of rasterize_gaussians_backward_records with R on the device; the
+    deterministic variant under `torch.use_deterministic_algorithms(True)`, as in `_backward`."""
+    lib = _capi.load()
+    device = colors.device
+    P = int(colors.shape[0])
+    H, W = int(dL_dout_color.size(1)), int(dL_dout_color.size(2))
+    det_buffer, det_bytes = None, 0
+    if torch.are_deterministic_algorithms_enabled():
+        n = C.c_size_t()
+        _capi.check(lib.gh_backward_det_workspace_size(P, int(capacity), C.byref(n)))
+        det_buffer, det_bytes = torch.empty(n.value, dtype=torch.uint8, device=device), n.value
+    with torch.cuda.device(device):
+        _capi.check(lib.gh_backward_capturable(
+            P, W, H, int(capacity), _ptr(_prep(background, "background", device)),
+            _ptr(_prep(colors, "colors", device, align=8)), _ptr(radii), _ptr(geomBuffer), _ptr(binningBuffer),
+            _ptr(imgBuffer), _ptr(_prep(dL_dout_color, "dL_dout_color", device)), 0, _stream(device),
+            _ptr(det_buffer), det_bytes))
 
 
 def alloc_grad_arena(P: int, device: torch.device, zero: bool = True, storage: torch.Tensor | None = None):

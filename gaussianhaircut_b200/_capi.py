@@ -39,6 +39,9 @@ _PROJ_ARGS = [
     _p, _p, _p,                              # viewmatrix projmatrix campos
     _f, _f, _f, _i, C.c_uint, _f]            # tan_fovx tan_fovy scale_modifier sh_degree flags det_eps
 
+# the same for the capturable variants: one device pointer to tan(fov / 2) (x, y) instead of the two host floats
+_PROJ_ARGS_CAPTURABLE = _PROJ_ARGS[:15] + [_p] + _PROJ_ARGS[17:]
+
 # name -> (restype, argtypes); every symbol declared in include/gh_rasterizer.h
 SIGNATURES = {
     "gh_abi_version": (_i, []),
@@ -100,6 +103,19 @@ SIGNATURES = {
         _p, _p, _p, _p, _p, _p,              # d_xyz d_scaling d_rotation d_dirs d_features_dc d_features_rest
         _p, _p, _p, _p, _p,                  # d_opacity d_label d_orient_conf d_means2D d_camera
         _p, _p, _p]),                        # nan_flag workspace stream
+    "gh_project_forward_binned_capturable": (_i, _PROJ_ARGS_CAPTURABLE + [
+        _p, _p, _p, _p, _p,                  # means2D colors opacities conic visible
+        _p, _p, _p, _p, _ll,                 # radii geom_buffer img_buffer binning_buffer capacity
+        _p, _p, _i, _p]),                    # status num_rendered debug stream
+    "gh_forward_render_capturable": (_i, [_i, _i, _i, _ll, _p, _p, _p, _p, _p, _p, _i, _p]),
+    "gh_backward_capturable": (_i, [_i, _i, _i, _ll, _p, _p, _p, _p, _p, _p, _p, _i, _p, _p, _sz]),
+    "gh_project_backward_capturable": (_i, _PROJ_ARGS_CAPTURABLE + [
+        _p, _p,                              # visible geom_buffer
+        _p, _p, _p, _p,                      # dL_dmeans2D dL_dconic dL_dcolors dL_dopacity
+        _p, _p, _p, _p, _p, _p,              # d_xyz d_scaling d_rotation d_dirs d_features_dc d_features_rest
+        _p, _p, _p, _p, _p,                  # d_opacity d_label d_orient_conf d_means2D d_camera
+        _p, _p, _i, _p]),                    # nan_flag workspace debug stream
+    "gh_adam_step_capturable": (_i, [_i, _p, _p, _p, _p, _p, _p, _f, _f, _f, _p, _p, _p, _i, _p]),
     "gh_strand_midpoints": (_i, [_i, _i, _p, _p, _p, _p]),          # S L origins dirs xyz stream
     "gh_strand_backward": (_i, [_i, _i, _p, _p, _p, _p]),           # S L d_xyz d_dirs nan_flag stream
     "gh_densify_classify": (_i, [_i, _p, _p, _p, _p, _f, _f, _f, _f, _p, _p]),

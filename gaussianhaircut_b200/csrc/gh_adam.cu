@@ -59,10 +59,12 @@ gh_adam_nan_kernel(GhAdamGroups g, unsigned int* __restrict__ flag)
     if (__any_sync(0xffffffffu, bad) && (threadIdx.x & 31) == 0) atomicOr(flag, 1u);
 }
 
-__global__ void __launch_bounds__(256)
-gh_adam_update_kernel(GhAdamGroups g, float beta1, float beta2, float eps,
-                      float bc1, float bc2_sqrt, const unsigned int* __restrict__ flag,
-                      const unsigned int* __restrict__ skip_flag, int* step_state)
+// DEV_LR: the learning rates are read from device memory (lr_dev[group]) instead of the launch argument
+template <bool DEV_LR>
+__device__ __forceinline__ void
+gh_adam_update_body(const GhAdamGroups& g, const float* __restrict__ lr_dev, float beta1, float beta2, float eps,
+                    float bc1, float bc2_sqrt, const unsigned int* __restrict__ flag,
+                    const unsigned int* __restrict__ skip_flag, int* step_state)
 {
     if (flag != nullptr && *flag != 0u) return;     // a gradient held a NaN: skip this step entirely
     if (skip_flag != nullptr && *skip_flag != 0u) return;   // the producer of the gradients reported a failure
@@ -80,7 +82,7 @@ gh_adam_update_kernel(GhAdamGroups g, float beta1, float beta2, float eps,
     float* __restrict__ V = g.exp_avg_sq[k];
     GhAdamConst c;
     c.beta1 = beta1; c.beta2 = beta2; c.omb1 = 1.0f - beta1; c.omb2 = 1.0f - beta2; c.eps = eps;
-    c.inv_bc2s = 1.0f / bc2_sqrt; c.step_size = g.lr[k] / bc1;
+    c.inv_bc2s = 1.0f / bc2_sqrt; c.step_size = (DEV_LR ? lr_dev[k] : g.lr[k]) / bc1;
     const unsigned long long tid = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
     const unsigned long long nthreads = (unsigned long long)gridDim.x * blockDim.x;
     unsigned long long done = 0;
@@ -113,7 +115,51 @@ gh_adam_update_kernel(GhAdamGroups g, float beta1, float beta2, float eps,
     }
 }
 
+__global__ void __launch_bounds__(256)
+gh_adam_update_kernel(GhAdamGroups g, float beta1, float beta2, float eps,
+                      float bc1, float bc2_sqrt, const unsigned int* __restrict__ flag,
+                      const unsigned int* __restrict__ skip_flag, int* step_state)
+{
+    gh_adam_update_body<false>(g, nullptr, beta1, beta2, eps, bc1, bc2_sqrt, flag, skip_flag, step_state);
+}
+
+// gh_adam_step_capturable: learning rates from device memory, step count always on the device
+__global__ void __launch_bounds__(256)
+gh_adam_update_dev_lr_kernel(GhAdamGroups g, const float* __restrict__ lrs, float beta1, float beta2, float eps,
+                             const unsigned int* __restrict__ flag, const unsigned int* __restrict__ skip_flag,
+                             int* step_state)
+{
+    gh_adam_update_body<true>(g, lrs, beta1, beta2, eps, 0.f, 0.f, flag, skip_flag, step_state);
+}
+
 }  // namespace
+
+// the kernel-argument view of the caller's HOST arrays (no launch); GH_OK or GH_E_INVALID_ARG
+// one grid row per group; enough CTAs per row for the largest group to fill the machine
+static int gh_adam_groups(const char* who, int n_groups, float* const* params, const float* const* grads,
+                          float* const* exp_avg, float* const* exp_avg_sq, const unsigned long long* sizes,
+                          const float* lrs_host, GhAdamGroups& g, unsigned long long& total, dim3& grid)
+{
+    total = 0;
+    for (int k = 0; k < GH_ADAM_MAX_GROUPS; k++) {
+        const bool on = k < n_groups;
+        g.param[k] = on ? params[k] : nullptr; g.grad[k] = on ? grads[k] : nullptr;
+        g.exp_avg[k] = on ? exp_avg[k] : nullptr; g.exp_avg_sq[k] = on ? exp_avg_sq[k] : nullptr;
+        g.lr[k] = (on && lrs_host) ? lrs_host[k] : 0.f;
+        if (on) {
+            if (!params[k] || !grads[k] || !exp_avg[k] || !exp_avg_sq[k])
+                return gh_set_error(GH_E_INVALID_ARG, "%s: NULL parameter / gradient / moment pointer", who);
+            total += sizes[k];
+        }
+        g.end[k] = total;
+    }
+    g.n = n_groups;
+    unsigned long long largest = 0;
+    for (int k = 0; k < n_groups; k++) largest = sizes[k] > largest ? sizes[k] : largest;
+    const unsigned long long want = (largest / 4 + 255) / 256;
+    grid = dim3((unsigned int)(want < 1 ? 1 : (want > 132ull * 8 ? 132ull * 8 : want)), (unsigned int)n_groups);
+    return GH_OK;
+}
 
 extern "C" int gh_adam_step(int n_groups, float* const* params, const float* const* grads,
                             float* const* exp_avg, float* const* exp_avg_sq,
@@ -126,28 +172,12 @@ extern "C" int gh_adam_step(int n_groups, float* const* params, const float* con
     if (n_groups <= 0 || n_groups > GH_ADAM_MAX_GROUPS || (step < 1 && step_state == nullptr) || !params || !grads || !exp_avg || !exp_avg_sq || !sizes || !lrs)
         return gh_set_error(GH_E_INVALID_ARG, "gh_adam_step: bad group count / step or missing array");
     GhAdamGroups g;
-    unsigned long long total = 0;
-    for (int k = 0; k < GH_ADAM_MAX_GROUPS; k++) {
-        const bool on = k < n_groups;
-        g.param[k] = on ? params[k] : nullptr; g.grad[k] = on ? grads[k] : nullptr;
-        g.exp_avg[k] = on ? exp_avg[k] : nullptr; g.exp_avg_sq[k] = on ? exp_avg_sq[k] : nullptr;
-        g.lr[k] = on ? lrs[k] : 0.f;
-        if (on) {
-            if (!params[k] || !grads[k] || !exp_avg[k] || !exp_avg_sq[k])
-                return gh_set_error(GH_E_INVALID_ARG, "gh_adam_step: NULL parameter / gradient / moment pointer");
-            total += sizes[k];
-        }
-        g.end[k] = total;
-    }
-    g.n = n_groups;
-    if (total == 0) return GH_OK;
+    unsigned long long total;
+    dim3 grid;
+    const int rc = gh_adam_groups("gh_adam_step", n_groups, params, grads, exp_avg, exp_avg_sq, sizes, lrs, g, total, grid);
+    if (rc != GH_OK || total == 0) return rc;
     const double bc1 = 1.0 - pow((double)beta1, (double)(step < 1 ? 1 : step));
     const double bc2 = 1.0 - pow((double)beta2, (double)(step < 1 ? 1 : step));
-    // one grid row per group; enough CTAs per row for the largest group to fill the machine
-    unsigned long long largest = 0;
-    for (int k = 0; k < n_groups; k++) largest = sizes[k] > largest ? sizes[k] : largest;
-    const unsigned long long want = (largest / 4 + 255) / 256;
-    const dim3 grid((unsigned int)(want < 1 ? 1 : (want > 132ull * 8 ? 132ull * 8 : want)), (unsigned int)n_groups);
     if (nan_flag) {
         const cudaError_t e = cudaMemsetAsync(nan_flag, 0, sizeof(unsigned int), stream);
         if (e != cudaSuccess) return gh_cuda_status("gh_adam_step", "memset(NaN flag)", e);
@@ -155,4 +185,33 @@ extern "C" int gh_adam_step(int n_groups, float* const* params, const float* con
     }
     gh_adam_update_kernel<<<grid, 256, 0, stream>>>(g, beta1, beta2, eps, (float)bc1, (float)sqrt(bc2), nan_flag, skip_flag, step_state);
     return gh_launch_status("gh_adam_step", nan_flag ? 2 : 1);
+}
+
+extern "C" int gh_adam_step_capturable(int n_groups, float* const* params, const float* const* grads,
+                                       float* const* exp_avg, float* const* exp_avg_sq,
+                                       const unsigned long long* sizes, const float* lrs,
+                                       float beta1, float beta2, float eps, int* step_state,
+                                       unsigned int* nan_flag, const unsigned int* skip_flag, int debug, gh_stream_t stream_)
+{
+    const char* who = "gh_adam_step_capturable";
+    cudaStream_t stream = (cudaStream_t)stream_;
+    gh_clear_error();
+    int rc = gh_check_capturable(who, debug);
+    if (rc != GH_OK) return rc;
+    if (n_groups <= 0 || n_groups > GH_ADAM_MAX_GROUPS || !params || !grads || !exp_avg || !exp_avg_sq || !sizes)
+        return gh_set_error(GH_E_INVALID_ARG, "%s: bad group count or missing array", who);
+    if (!lrs) return gh_set_error(GH_E_INVALID_ARG, "%s: lrs (device float[n_groups]) is required", who);
+    if (!step_state) return gh_set_error(GH_E_INVALID_ARG, "%s: step_state (device int[2]) is required", who);
+    GhAdamGroups g;
+    unsigned long long total;
+    dim3 grid;
+    rc = gh_adam_groups(who, n_groups, params, grads, exp_avg, exp_avg_sq, sizes, nullptr, g, total, grid);
+    if (rc != GH_OK || total == 0) return rc;
+    if (nan_flag) {
+        rc = gh_cuda_status(who, "memset(NaN flag)", cudaMemsetAsync(nan_flag, 0, sizeof(unsigned int), stream));
+        if (rc != GH_OK) return rc;
+        gh_adam_nan_kernel<<<grid, 256, 0, stream>>>(g, nan_flag);
+    }
+    gh_adam_update_dev_lr_kernel<<<grid, 256, 0, stream>>>(g, lrs, beta1, beta2, eps, nan_flag, skip_flag, step_state);
+    return gh_launch_status(who, nan_flag ? 2 : 1);
 }

@@ -183,6 +183,37 @@ int gh_forward_phase1(const char* who, int P, int width, int height, char* geom_
     return GH_OK;
 }
 
+int gh_check_capturable(const char* who, int debug)
+{
+    if (debug != 0) return gh_set_error(GH_E_INVALID_ARG, "%s: debug mode synchronises after every stage and cannot be captured", who);
+    if (g_timing.load()) return gh_set_error(GH_E_INVALID_ARG, "%s: the stage timer synchronises after every stage; disable it (gh_stage_timing_enable(0))", who);
+    return GH_OK;
+}
+
+int gh_check_capacity(const char* who, long long capacity)
+{
+    if (capacity < 0 || capacity > 0xffffffffll) return gh_set_error(GH_E_INVALID_ARG, "%s: capacity must lie in [0, 2^32)", who);
+    return GH_OK;
+}
+
+int gh_forward_phase1_capturable(const char* who, int P, int width, int height, int* radii, char* geom_buffer,
+                                 char* img_buffer, char* binning_buffer, long long capacity, unsigned int* status,
+                                 unsigned int* num_rendered_out, cudaStream_t stream, GhBinLaunch launch, const void* bin)
+{
+    int gx, gy; const int T = gh_tile_grid(width, height, gx, gy);
+    if ((unsigned long long)gx * gx * gy >= (1ull << 32))      // exactness bound of the tile enumeration (gh_warp_rects)
+        return gh_set_error(GH_E_INVALID_ARG, "%s: image too large (tile grid gx * gx * gy must stay below 2^32)", who);
+    GhGeomWS geom = GhGeomWS::carve(geom_buffer, (size_t)P);
+    GhImgWS img = GhImgWS::carve(img_buffer, (size_t)width * height, (size_t)T);
+    int rc = gh_cuda_status(who, "memset(tile histogram)", cudaMemsetAsync(img.ctrl, 0, 256 + gh_align_up((size_t)T * 4, 256), stream));
+    if (rc != GH_OK) return rc;
+    launch(bin, geom, img, gx, gy);
+    gh_launch_tile_scan(T, img, stream);
+    gh_launch_capacity_guard(P, radii, T, img, (unsigned int)capacity, status, num_rendered_out, stream);
+    gh_launch_emit(P, radii, geom, img, GhBinWS::carve(binning_buffer, (size_t)capacity), (unsigned int)capacity, gx, gy, stream);
+    return gh_launch_status(who, 3);
+}
+
 extern "C" {
 
 int gh_abi_version(void) { return 5; }
@@ -408,6 +439,70 @@ int gh_backward(
     }
     GH_STAGE("gh_backward", stream, debug, "preprocess backward");
     return GH_OK;
+}
+
+int gh_forward_render_capturable(
+    int P, int width, int height, long long capacity,
+    const float* background, const float* colors_precomp,
+    char* geom_buffer, char* binning_buffer, char* img_buffer,
+    float* out_color, int debug, gh_stream_t stream_)
+{
+    const char* who = "gh_forward_render_capturable";
+    cudaStream_t stream = (cudaStream_t)stream_;
+    gh_clear_error();
+    int rc = gh_check_capturable(who, debug);
+    if (rc == GH_OK) rc = gh_check_capacity(who, capacity);
+    if (rc != GH_OK) return rc;
+    if (P <= 0 || width <= 0 || height <= 0) return gh_set_error(GH_E_INVALID_ARG, "%s: bad sizes", who);
+    if (!background || !colors_precomp || !geom_buffer || !binning_buffer || !img_buffer || !out_color)
+        return gh_set_error(GH_E_INVALID_ARG, "%s: missing mandatory pointer", who);
+    int gx, gy; const int T = gh_tile_grid(width, height, gx, gy);
+    GhGeomWS geom = GhGeomWS::carve(geom_buffer, (size_t)P);
+    GhImgWS img = GhImgWS::carve(img_buffer, (size_t)width * height, (size_t)T);
+    GhBinWS bin = GhBinWS::carve(binning_buffer, (size_t)capacity);
+    const int n = gh_launch_tile_sort_capturable(T, (unsigned int)capacity, img, bin, stream);
+    gh_launch_blend_forward(width, height, gx, gy, geom, img, bin, colors_precomp, background, out_color, stream);
+    return gh_launch_status(who, n + 1);
+}
+
+int gh_backward_capturable(
+    int P, int width, int height, long long capacity,
+    const float* background, const float* colors_precomp, const int* radii,
+    char* geom_buffer, char* binning_buffer, char* img_buffer,
+    const float* dL_dpix, int debug, gh_stream_t stream_, char* det_buffer, size_t det_bytes)
+{
+    const char* who = "gh_backward_capturable";
+    cudaStream_t stream = (cudaStream_t)stream_;
+    gh_clear_error();
+    int rc = gh_check_capturable(who, debug);
+    if (rc == GH_OK) rc = gh_check_capacity(who, capacity);
+    if (rc != GH_OK) return rc;
+    if (P <= 0 || width <= 0 || height <= 0) return gh_set_error(GH_E_INVALID_ARG, "%s: bad sizes", who);
+    if (det_buffer == nullptr && det_bytes != 0)
+        return gh_set_error(GH_E_INVALID_ARG, "%s: det_bytes given without a det_buffer", who);
+    if (det_buffer != nullptr && det_bytes < GhDetWS::bytes((size_t)P, (size_t)capacity))
+        return gh_set_error(GH_E_INVALID_ARG, "%s: det_buffer smaller than gh_backward_det_workspace_size(P, capacity)", who);
+    if (!background || !colors_precomp || !radii || !geom_buffer || !binning_buffer || !img_buffer || !dL_dpix)
+        return gh_set_error(GH_E_INVALID_ARG, "%s: missing mandatory pointer", who);
+    if (((size_t)colors_precomp & 7)) return gh_set_error(GH_E_INVALID_ARG, "colors_precomp must be 8-byte aligned");
+    int gx, gy; const int T = gh_tile_grid(width, height, gx, gy);
+    GhGeomWS geom = GhGeomWS::carve(geom_buffer, (size_t)P);
+    GhImgWS img = GhImgWS::carve(img_buffer, (size_t)width * height, (size_t)T);
+    GhBinWS bin = GhBinWS::carve(binning_buffer, (size_t)capacity);
+    // no R == 0 branch: an empty (or overflowed, see gh_launch_capacity_guard) frame has no instance in any tile, and
+    // both variants then leave zero records
+    if (det_buffer != nullptr) {
+        // deterministic: the row offsets come from the radii, so off[P] = R <= capacity rows
+        GhDetWS det = GhDetWS::carve(det_buffer, (size_t)P, (size_t)capacity);
+        const int n = gh_launch_det_offsets(P, gx, gy, radii, geom, det, stream);
+        gh_launch_blend_backward_det(width, height, gx, gy, radii, geom, img, bin, det, colors_precomp, background, dL_dpix, stream);
+        gh_launch_det_gather(P, geom, det, stream);
+        return gh_launch_status(who, n + 2);
+    }
+    rc = gh_cuda_status(who, "memset(accumulation records)", cudaMemsetAsync(geom.acc16, 0, (size_t)P * 64, stream));
+    if (rc != GH_OK) return rc;
+    gh_launch_blend_backward(width, height, gx, gy, geom, img, bin, colors_precomp, background, dL_dpix, stream);
+    return gh_launch_status(who, 1);
 }
 
 int gh_mark_visible(int P, const float* means3D, const float* viewmatrix, const float* projmatrix,

@@ -14,6 +14,7 @@
 #include <cooperative_groups.h>
 #include "gh_common.cuh"
 #include "gh_kernels.h"
+#include "../../include/gh_rasterizer.h"
 
 namespace {
 
@@ -342,6 +343,26 @@ gh_segment_sort_kernel(const uint2* __restrict__ seg, const GhCtrl* __restrict__
     }
 }
 
+// ---------------------------------------------------------------- capacity guard (capturable forward)
+// Runs between the tile scan and emit.  R fits: nothing to do (every CTA leaves after one load of ctrl).  R exceeds the
+// capacity of the binning buffer: emit writes nothing (its own test), and this kernel empties the frame -- every tile
+// range (0, 0), every radius 0 -- so that the sort, both blend kernels, the deterministic row offsets and the
+// densification statistics all see a frame with no instance: background image, zero records, zero gradients.
+__global__ void __launch_bounds__(256)
+gh_capacity_guard_kernel(int P, int* __restrict__ radii, int T, uint2* __restrict__ ranges, const GhCtrl* __restrict__ ctrl,
+                         uint32_t capacity, unsigned int* __restrict__ status, unsigned int* __restrict__ r_out)
+{
+    const uint32_t R = ctrl->num_rendered;
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        if (r_out) *r_out = R;
+        if (R > capacity) atomicOr(status, GH_STATUS_BINNING_OVERFLOW);
+    }
+    if (R <= capacity) return;
+    const int stride = gridDim.x * blockDim.x;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < T; i += stride) ranges[i] = make_uint2(0u, 0u);
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < P; i += stride) radii[i] = 0;
+}
+
 }  // namespace
 
 void gh_launch_tile_scan(int T, GhImgWS img, cudaStream_t stream)
@@ -363,6 +384,22 @@ int gh_launch_tile_sort(int T, unsigned int max_tile_len, long long R, GhImgWS i
     if (max_tile_len <= GH_INKERNEL_SORT_MAX) return 0;
     gh_tile_split_long_kernel<<<T, 256, 0, stream>>>(img.ranges, bin.inst, bin.tmp, bin.seg, img.ctrl, GH_INKERNEL_SORT_MAX);
     const unsigned int nseg_max = (unsigned int)GhBinWS::max_segments((size_t)R);   // >= sum over long tiles of ceil(n/768)
+    gh_segment_sort_kernel<<<nseg_max, 256, 0, stream>>>(bin.seg, img.ctrl, bin.inst, bin.tmp);
+    return 2;
+}
+
+void gh_launch_capacity_guard(int P, int* radii, int T, GhImgWS img, unsigned int capacity, unsigned int* status,
+                              unsigned int* num_rendered_out, cudaStream_t stream)
+{
+    gh_capacity_guard_kernel<<<2 * 132, 256, 0, stream>>>(P, radii, T, img.ranges, img.ctrl, capacity, status, num_rendered_out);
+}
+
+int gh_launch_tile_sort_capturable(int T, unsigned int capacity, GhImgWS img, GhBinWS bin, cudaStream_t stream)
+{
+    // max_tile_len is only known on the device: the split always runs (a CTA whose list is short leaves at once), and the
+    // segment sort gets the grid of the largest R that fits (R <= capacity, hence nseg <= max_segments(capacity))
+    gh_tile_split_long_kernel<<<T, 256, 0, stream>>>(img.ranges, bin.inst, bin.tmp, bin.seg, img.ctrl, GH_INKERNEL_SORT_MAX);
+    const unsigned int nseg_max = (unsigned int)GhBinWS::max_segments((size_t)capacity);
     gh_segment_sort_kernel<<<nseg_max, 256, 0, stream>>>(bin.seg, img.ctrl, bin.inst, bin.tmp);
     return 2;
 }

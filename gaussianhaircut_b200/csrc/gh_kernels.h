@@ -22,6 +22,16 @@ void gh_launch_emit(int P, const int* radii, GhGeomWS geom, GhImgWS img, GhBinWS
 // returns the number of kernels launched
 int gh_launch_tile_sort(int T, unsigned int max_tile_len, long long R, GhImgWS img, GhBinWS bin, cudaStream_t stream);
 
+// The capturable forward (R only on the device, a binning buffer of `capacity` records):
+//  - capacity guard, right behind the tile scan: when R > capacity it ORs GH_STATUS_BINNING_OVERFLOW into *status and
+//    turns the frame into an empty one -- every tile range (0, 0) and every radius 0 -- so that no later kernel reads
+//    or writes a record at or beyond `capacity`; *num_rendered_out (may be NULL) receives R either way;
+//  - the long-list sort with grids bounded by T and `capacity` (its CTAs exit when their list is short); returns the
+//    number of kernels launched.
+void gh_launch_capacity_guard(int P, int* radii, int T, GhImgWS img, unsigned int capacity, unsigned int* status,
+                              unsigned int* num_rendered_out, cudaStream_t stream);
+int gh_launch_tile_sort_capturable(int T, unsigned int capacity, GhImgWS img, GhBinWS bin, cudaStream_t stream);
+
 void gh_launch_blend_forward(int W, int H, int gx, int gy, GhGeomWS geom, GhImgWS img, GhBinWS bin,
                              const float* features, const float* bg, float* out_color,
                              cudaStream_t stream);
@@ -79,6 +89,26 @@ int gh_forward_phase1(const char* who, int P, int width, int height, char* geom_
 }
 // argument checks of the optional binning buffer of the first-phase entry points (before any launch)
 int gh_check_phase1_bin(const char* who, const GhPhase1Bin& emit);
+
+// The first phase of the capturable forward (gh_project_forward_binned_capturable): as gh_forward_phase1, but nothing is
+// read back and emit always goes into the caller's buffer of `capacity` records, behind the capacity guard
+// (gh_launch_capacity_guard).  No host synchronisation, no allocation.
+int gh_forward_phase1_capturable(const char* who, int P, int width, int height, int* radii, char* geom_buffer,
+                                 char* img_buffer, char* binning_buffer, long long capacity, unsigned int* status,
+                                 unsigned int* num_rendered_out, cudaStream_t stream, GhBinLaunch launch, const void* bin);
+template <class F>
+int gh_forward_phase1_capturable(const char* who, int P, int width, int height, int* radii, char* geom_buffer,
+                                 char* img_buffer, char* binning_buffer, long long capacity, unsigned int* status,
+                                 unsigned int* num_rendered_out, cudaStream_t stream, const F& bin) {
+    return gh_forward_phase1_capturable(who, P, width, height, radii, geom_buffer, img_buffer, binning_buffer, capacity,
+                                        status, num_rendered_out, stream,
+                                        [](const void* f, const GhGeomWS& g, const GhImgWS& i, int gx, int gy) { (*static_cast<const F*>(f))(g, i, gx, gy); }, &bin);
+}
+// shared refusals of every capturable entry point (before any launch): debug != 0 and calls while the stage timer is on
+// (both synchronise with the host)
+int gh_check_capturable(const char* who, int debug);
+// the binning capacity argument of the capturable entry points: [0, 2^32)
+int gh_check_capacity(const char* who, long long capacity);
 
 // per-thread error message behind gh_last_error(): every extern "C" entry point clears it on entry and
 // sets it before returning a GH_E_* code (defined in gh_api.cu).  gh_set_error is its only writer (printf-style,

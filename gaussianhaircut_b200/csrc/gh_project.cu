@@ -69,12 +69,12 @@ __device__ __forceinline__ void gh_rest_store(const float* s_rest, float* __rest
 // as gh_preprocess_kernel (gh_common.cuh), hence bit-identical radii / records / keys.
 // STRAND: Gaussian i is a polyline segment whose scales and rotation come from dirs[i] (gh_proj_geometry).
 template <bool BIN, bool STRAND>
-__global__ void __launch_bounds__(GH_PJ_THREADS)
-gh_project_forward_kernel(GhProjArgs A, float* __restrict__ means2D, float* __restrict__ colors,
-                          float* __restrict__ opac_out, float* __restrict__ conic_out, float* __restrict__ cov3D_out,
-                          unsigned char* __restrict__ mask_out,
-                          int* __restrict__ radii, GhGeo* __restrict__ geo, float* __restrict__ depth,
-                          uint32_t* __restrict__ tile_count, int gx, int gy)
+__device__ __forceinline__ void
+gh_project_forward_body(const GhProjArgs& A, float* __restrict__ means2D, float* __restrict__ colors,
+                        float* __restrict__ opac_out, float* __restrict__ conic_out, float* __restrict__ cov3D_out,
+                        unsigned char* __restrict__ mask_out,
+                        int* __restrict__ radii, GhGeo* __restrict__ geo, float* __restrict__ depth,
+                        uint32_t* __restrict__ tile_count, int gx, int gy)
 {
     __shared__ __align__(16) float s_rest[GH_PJ_THREADS * GH_PJ_REST];
     const int row0 = blockIdx.x * GH_PJ_THREADS;
@@ -116,6 +116,31 @@ gh_project_forward_kernel(GhProjArgs A, float* __restrict__ means2D, float* __re
     if (BIN) gh_warp_tile_histogram(rect_minx, rect_miny, rect_maxx, rect_maxy, gx, tile_count);
 }
 
+template <bool BIN, bool STRAND>
+__global__ void __launch_bounds__(GH_PJ_THREADS)
+gh_project_forward_kernel(GhProjArgs A, float* __restrict__ means2D, float* __restrict__ colors,
+                          float* __restrict__ opac_out, float* __restrict__ conic_out, float* __restrict__ cov3D_out,
+                          unsigned char* __restrict__ mask_out,
+                          int* __restrict__ radii, GhGeo* __restrict__ geo, float* __restrict__ depth,
+                          uint32_t* __restrict__ tile_count, int gx, int gy)
+{
+    gh_project_forward_body<BIN, STRAND>(A, means2D, colors, opac_out, conic_out, cov3D_out, mask_out, radii, geo, depth,
+                                         tile_count, gx, gy);
+}
+
+// The capturable first phase (gh_project_forward_binned_capturable): tan(fov / 2) is read from device memory, so that a
+// captured launch serves every camera.  GaussianModel rows only.
+__global__ void __launch_bounds__(GH_PJ_THREADS)
+gh_project_forward_tan_kernel(GhProjArgs A, const float* __restrict__ tan_fov, float* __restrict__ means2D,
+                              float* __restrict__ colors, float* __restrict__ opac_out, float* __restrict__ conic_out,
+                              unsigned char* __restrict__ mask_out, int* __restrict__ radii, GhGeo* __restrict__ geo,
+                              float* __restrict__ depth, uint32_t* __restrict__ tile_count, int gx, int gy)
+{
+    A.tanx = __ldg(tan_fov); A.tany = __ldg(tan_fov + 1);
+    gh_project_forward_body<true, false>(A, means2D, colors, opac_out, conic_out, nullptr, mask_out, radii, geo, depth,
+                                         tile_count, gx, gy);
+}
+
 // ------------------------------------------------------------------------------------------------ backward
 // Incoming gradients: either the four API-shaped tensors of gh_backward (dL_dmean2D (P,3) NDC units,
 // dL_dconic (P,4) = (d/da, HALF d/db, unused, d/dc), dL_dcolor (P,10), dL_dopacity (P)), or -- when acc16 is
@@ -123,8 +148,8 @@ gh_project_forward_kernel(GhProjArgs A, float* __restrict__ means2D, float* __re
 // opacity), which skips the unpack kernel and its round trip through HBM.
 // STRAND: the scale and rotation gradients are folded into d_dirs in registers; d_scaling / d_rotation are not written.
 template <bool STRAND>
-__global__ void __launch_bounds__(GH_PJ_THREADS)
-gh_project_backward_kernel(GhProjArgs A, const unsigned char* __restrict__ mask,
+__device__ __forceinline__ void
+gh_project_backward_body(const GhProjArgs& A, const unsigned char* __restrict__ mask,
                            const float* __restrict__ acc16,
                            const float* __restrict__ g_mean2D, const float* __restrict__ g_conic4,
                            const float* __restrict__ g_color, const float* __restrict__ g_opacity,
@@ -263,6 +288,44 @@ gh_project_backward_kernel(GhProjArgs A, const unsigned char* __restrict__ mask,
         d_cam[16 + 2] = 0.f; d_cam[16 + 6] = 0.f; d_cam[16 + 10] = 0.f; d_cam[16 + 14] = 0.f;
         *cam_ticket = 0u;
     }
+}
+
+template <bool STRAND>
+__global__ void __launch_bounds__(GH_PJ_THREADS)
+gh_project_backward_kernel(GhProjArgs A, const unsigned char* __restrict__ mask,
+                           const float* __restrict__ acc16,
+                           const float* __restrict__ g_mean2D, const float* __restrict__ g_conic4,
+                           const float* __restrict__ g_color, const float* __restrict__ g_opacity,
+                           float* __restrict__ d_xyz, float* __restrict__ d_scaling, float* __restrict__ d_rotation,
+                           float* __restrict__ d_dirs, float* __restrict__ d_fdc, float* __restrict__ d_frest,
+                           float* __restrict__ d_opacity, float* __restrict__ d_label, float* __restrict__ d_conf,
+                           float* __restrict__ d_mean2D_out,
+                           float* __restrict__ cam_partial, unsigned int* __restrict__ cam_ticket,
+                           float* __restrict__ d_cam, unsigned int* __restrict__ nan_flag)
+{
+    gh_project_backward_body<STRAND>(A, mask, acc16, g_mean2D, g_conic4, g_color, g_opacity, d_xyz, d_scaling, d_rotation,
+                                     d_dirs, d_fdc, d_frest, d_opacity, d_label, d_conf, d_mean2D_out, cam_partial,
+                                     cam_ticket, d_cam, nan_flag);
+}
+
+// gh_project_backward_capturable: tan(fov / 2) from device memory, as in gh_project_forward_tan_kernel
+template <bool STRAND>
+__global__ void __launch_bounds__(GH_PJ_THREADS)
+gh_project_backward_tan_kernel(GhProjArgs A, const float* __restrict__ tan_fov, const unsigned char* __restrict__ mask,
+                               const float* __restrict__ acc16,
+                               const float* __restrict__ g_mean2D, const float* __restrict__ g_conic4,
+                               const float* __restrict__ g_color, const float* __restrict__ g_opacity,
+                               float* __restrict__ d_xyz, float* __restrict__ d_scaling, float* __restrict__ d_rotation,
+                               float* __restrict__ d_dirs, float* __restrict__ d_fdc, float* __restrict__ d_frest,
+                               float* __restrict__ d_opacity, float* __restrict__ d_label, float* __restrict__ d_conf,
+                               float* __restrict__ d_mean2D_out,
+                               float* __restrict__ cam_partial, unsigned int* __restrict__ cam_ticket,
+                               float* __restrict__ d_cam, unsigned int* __restrict__ nan_flag)
+{
+    A.tanx = __ldg(tan_fov); A.tany = __ldg(tan_fov + 1);
+    gh_project_backward_body<STRAND>(A, mask, acc16, g_mean2D, g_conic4, g_color, g_opacity, d_xyz, d_scaling, d_rotation,
+                                     d_dirs, d_fdc, d_frest, d_opacity, d_label, d_conf, d_mean2D_out, cam_partial,
+                                     cam_ticket, d_cam, nan_flag);
 }
 
 int gh_proj_check(GhProjArgs& A, const char* who, bool strand)
@@ -422,4 +485,95 @@ extern "C" int gh_project_backward(
         d_xyz, d_scaling, d_rotation, d_dirs, d_features_dc, d_features_rest, d_opacity, d_label, d_orient_conf,
         d_means2D, partial, ticket, d_camera, nan_flag);
     return gh_launch_status("gh_project_backward", 1);
+}
+
+// ------------------------------------------------------------------------------------------------ capturable
+// gh_project_forward_binned and gh_project_backward with tan(fov / 2) read from device memory and R kept on the device:
+// every argument of a captured launch stays valid from one camera and one iteration to the next.
+extern "C" int gh_project_forward_binned_capturable(
+    int P, int width, int height,
+    const float* xyz, const float* scaling, const float* rotation, const float* dirs,
+    const float* features_dc, const float* features_rest,
+    const float* opacity, const float* label, const float* orient_conf,
+    const float* viewmatrix, const float* projmatrix, const float* campos,
+    const float* tan_fov, float scale_modifier, int sh_degree, unsigned int flags, float det_eps,
+    float* means2D, float* colors, float* opacities, float* conic, unsigned char* visible,
+    int* radii, char* geom_buffer, char* img_buffer, char* binning_buffer, long long capacity,
+    unsigned int* status, unsigned int* num_rendered, int debug, gh_stream_t stream_)
+{
+    const char* who = "gh_project_forward_binned_capturable";
+    cudaStream_t stream = (cudaStream_t)stream_;
+    gh_clear_error();
+    int rc = gh_check_capturable(who, debug);
+    if (rc == GH_OK) rc = gh_check_capacity(who, capacity);
+    if (rc != GH_OK) return rc;
+    if (!tan_fov) return gh_set_error(GH_E_INVALID_ARG, "%s: tan_fov (device float[2]) is required", who);
+    if (!status) return gh_set_error(GH_E_INVALID_ARG, "%s: status (device uint32) is required", who);
+    if (gh_proj_strand(flags)) return gh_set_error(GH_E_INVALID_ARG, "%s: strand mode is not supported", who);
+    // (the kernel reads tan(fov / 2) from tan_fov; 1 stands in for it in the host-side checks)
+    GhProjArgs A = gh_proj_args(P, width, height, xyz, scaling, rotation, dirs, features_dc, features_rest, opacity, label,
+                                orient_conf, viewmatrix, projmatrix, campos, 1.f, 1.f, scale_modifier, sh_degree, flags, det_eps);
+    rc = gh_proj_check(A, who, false);
+    if (rc != GH_OK) return rc;
+    if (!means2D || !colors || !opacities || !conic || !visible || !radii || !geom_buffer || !img_buffer || !binning_buffer)
+        return gh_set_error(GH_E_INVALID_ARG, "%s: missing output pointer", who);
+    if ((size_t)colors & 7) return gh_set_error(GH_E_INVALID_ARG, "%s: colors must be 8-byte aligned", who);
+    return gh_forward_phase1_capturable(who, P, width, height, radii, geom_buffer, img_buffer, binning_buffer, capacity,
+                                        status, num_rendered, stream, [&](const GhGeomWS& geom, const GhImgWS& img, int gx, int gy) {
+        gh_project_forward_tan_kernel<<<(P + GH_PJ_THREADS - 1) / GH_PJ_THREADS, GH_PJ_THREADS, 0, stream>>>(
+            A, tan_fov, means2D, colors, opacities, conic, visible, radii, geom.geo, geom.depth, img.tile_count, gx, gy);
+        gh_count_launches(1);
+    });
+}
+
+extern "C" int gh_project_backward_capturable(
+    int P, int width, int height,
+    const float* xyz, const float* scaling, const float* rotation, const float* dirs,
+    const float* features_dc, const float* features_rest,
+    const float* opacity, const float* label, const float* orient_conf,
+    const float* viewmatrix, const float* projmatrix, const float* campos,
+    const float* tan_fov, float scale_modifier, int sh_degree, unsigned int flags, float det_eps,
+    const unsigned char* visible,
+    const char* geom_buffer,
+    const float* dL_dmeans2D, const float* dL_dconic, const float* dL_dcolors, const float* dL_dopacity,
+    float* d_xyz, float* d_scaling, float* d_rotation, float* d_dirs, float* d_features_dc, float* d_features_rest,
+    float* d_opacity, float* d_label, float* d_orient_conf, float* d_means2D, float* d_camera,
+    unsigned int* nan_flag, void* workspace, int debug, gh_stream_t stream_)
+{
+    const char* who = "gh_project_backward_capturable";
+    cudaStream_t stream = (cudaStream_t)stream_;
+    gh_clear_error();
+    int rc = gh_check_capturable(who, debug);
+    if (rc != GH_OK) return rc;
+    if (!tan_fov) return gh_set_error(GH_E_INVALID_ARG, "%s: tan_fov (device float[2]) is required", who);
+    GhProjArgs A = gh_proj_args(P, width, height, xyz, scaling, rotation, dirs, features_dc, features_rest, opacity, label,
+                                orient_conf, viewmatrix, projmatrix, campos, 1.f, 1.f, scale_modifier, sh_degree, flags, det_eps);
+    const bool strand = gh_proj_strand(flags);
+    rc = gh_proj_check(A, who, strand);
+    if (rc != GH_OK) return rc;
+    if (strand && (d_scaling || d_rotation))
+        return gh_set_error(GH_E_INVALID_ARG, "%s: strand mode folds scale and rotation gradients into d_dirs, d_scaling / d_rotation must be NULL", who);
+    if (strand && !d_dirs) return gh_set_error(GH_E_INVALID_ARG, "%s: strand mode needs d_dirs", who);
+    if (!visible || !d_xyz || (!strand && (!d_scaling || !d_rotation)) || !d_features_dc || !d_features_rest)
+        return gh_set_error(GH_E_INVALID_ARG, "%s: missing mandatory pointer", who);
+    if (geom_buffer == nullptr && (!dL_dmeans2D || !dL_dconic || !dL_dcolors || !dL_dopacity))
+        return gh_set_error(GH_E_INVALID_ARG, "%s: pass the geometry workspace of the blend backward or the four incoming gradients", who);
+    if (((size_t)d_rotation & 15) || (dL_dconic && ((size_t)dL_dconic & 15)) || (dL_dcolors && ((size_t)dL_dcolors & 7)))
+        return gh_set_error(GH_E_INVALID_ARG, "%s: d_rotation / dL_dconic must be 16-byte, dL_dcolors 8-byte aligned", who);
+    if (d_camera != nullptr && (workspace == nullptr || ((size_t)workspace & 15)))
+        return gh_set_error(GH_E_INVALID_ARG, "%s: camera gradients need the 16-byte aligned workspace", who);
+    const float* acc16 = nullptr;
+    if (geom_buffer != nullptr) acc16 = GhGeomWS::carve(const_cast<char*>(geom_buffer), (size_t)P).acc16;
+    unsigned int* ticket = reinterpret_cast<unsigned int*>(workspace);
+    float* partial = workspace ? reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256) : nullptr;
+    if (d_camera != nullptr) {
+        rc = gh_cuda_status(who, "memset(ticket)", cudaMemsetAsync(ticket, 0, sizeof(unsigned int), stream));
+        if (rc != GH_OK) return rc;
+    }
+    auto kernel = strand ? gh_project_backward_tan_kernel<true> : gh_project_backward_tan_kernel<false>;
+    kernel<<<(P + GH_PJ_THREADS - 1) / GH_PJ_THREADS, GH_PJ_THREADS, 0, stream>>>(
+        A, tan_fov, visible, acc16, dL_dmeans2D, dL_dconic, dL_dcolors, dL_dopacity,
+        d_xyz, d_scaling, d_rotation, d_dirs, d_features_dc, d_features_rest, d_opacity, d_label, d_orient_conf,
+        d_means2D, partial, ticket, d_camera, nan_flag);
+    return gh_launch_status(who, 1);
 }

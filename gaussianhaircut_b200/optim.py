@@ -31,7 +31,7 @@ class FusedAdam:
     `.zero_grad()`, `.state_dict()` / `.load_state_dict()`.  All tensors float32 CUDA contiguous."""
 
     def __init__(self, param_groups: Iterable[Dict], betas=(0.9, 0.999), eps: float = 1e-15, nan_guard: bool = True,
-                 lr: float = 0.0):
+                 lr: float = 0.0, capturable: bool = False):
         self.param_groups: List[Dict] = []
         for g in param_groups:
             g = dict(g)
@@ -52,6 +52,10 @@ class FusedAdam:
         self.nan_flag = torch.zeros(1, dtype=torch.int32, device=dev) if nan_guard else None
         self.step_state = torch.zeros(2, dtype=torch.int32, device=dev)   # [steps taken, scratch], device resident
         self._keep = None
+        # capturable: the update reads the learning rates from this device tensor (one per parameter, in parameter order),
+        # so that a captured step follows a schedule; load_lrs() refreshes it from the groups' 'lr'
+        self.capturable = bool(capturable)
+        self.lrs = torch.zeros(len(flat), dtype=torch.float32, device=dev) if capturable else None
 
     # ------------------------------------------------------------------------------------------ helpers
     def _params(self) -> List[torch.Tensor]:
@@ -84,10 +88,18 @@ class FusedAdam:
                 elif p.grad is not None:
                     p.grad.zero_()
 
+    def load_lrs(self) -> None:
+        """Capturable mode: copy every group's 'lr' into the device tensor `lrs` (outside a CUDA-graph capture; step()
+        does it itself when it is not being captured)."""
+        vals = [float(g["lr"]) for g in self.param_groups for _ in g["params"]]
+        self.lrs.copy_(torch.tensor(vals, dtype=torch.float32))
+
     # ------------------------------------------------------------------------------------------ step
     def step(self, grads: Optional[Sequence[Optional[torch.Tensor]]] = None,
              skip_flags: Sequence[torch.Tensor] = (), nan_flag_in: Optional[torch.Tensor] = None):
         """Update every parameter that has a gradient (`grads` overrides `.grad`, in parameter order).
+        In capturable mode every parameter must have one, and the step neither reads the host learning rates nor
+        synchronises: it can be captured in a CUDA graph (gh_adam_step_capturable).
 
         `skip_flags`: device int32/uint32 tensors (1 element each; at most one is passed to the kernel, the
         others are OR-ed on the device first): the step is skipped when one is non-zero, e.g.
@@ -116,6 +128,8 @@ class FusedAdam:
                 ns.append(n); lrs.append(float(g["lr"]))
         if not ps:
             return
+        if self.capturable and len(ps) != len(self._params()):
+            raise RuntimeError("FusedAdam(capturable=True): every parameter needs a gradient")
         n = len(ps)
         arr = lambda ts: (C.c_void_p * n)(*[t.data_ptr() for t in ts])   # noqa: E731
         dev = ps[0].device
@@ -129,10 +143,18 @@ class FusedAdam:
             skip = torch.stack([f.reshape(-1)[0].to(torch.int32) for f in flags]).amax().reshape(1).contiguous()
         own_nan = self.nan_flag if nan_flag_in is None else None
         with torch.cuda.device(dev):
-            _capi.check(lib.gh_adam_step(
-                n, arr(ps), arr(gs), arr(ms), arr(vs), (C.c_ulonglong * n)(*ns), (C.c_float * n)(*lrs),
-                float(self.betas[0]), float(self.betas[1]), float(self.eps), 0,
-                _ptr(self.step_state), _ptr(own_nan), _ptr(skip), _stream(dev)))
+            if self.capturable:
+                if not torch.cuda.is_current_stream_capturing():
+                    self.load_lrs()
+                _capi.check(lib.gh_adam_step_capturable(
+                    n, arr(ps), arr(gs), arr(ms), arr(vs), (C.c_ulonglong * n)(*ns), _ptr(self.lrs),
+                    float(self.betas[0]), float(self.betas[1]), float(self.eps),
+                    _ptr(self.step_state), _ptr(own_nan), _ptr(skip), 0, _stream(dev)))
+            else:
+                _capi.check(lib.gh_adam_step(
+                    n, arr(ps), arr(gs), arr(ms), arr(vs), (C.c_ulonglong * n)(*ns), (C.c_float * n)(*lrs),
+                    float(self.betas[0]), float(self.betas[1]), float(self.eps), 0,
+                    _ptr(self.step_state), _ptr(own_nan), _ptr(skip), _stream(dev)))
         if nan_flag_in is not None:
             nan_flag_in.zero_()       # consumed: ready for the next iteration's backward (stream-ordered after the update)
         self._keep = (ps, gs, skip)   # keep the tensors alive until the kernels have run

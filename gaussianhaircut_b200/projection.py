@@ -91,6 +91,13 @@ def _common_args(pi: ProjectionInputs):
             pi.tanx, pi.tany, pi.mod, pi.sh_degree, pi.flags, pi.det_eps)
 
 
+def _common_args_capturable(pi: ProjectionInputs, tan_fov: torch.Tensor):
+    """_common_args with tan(fov / 2) from the device float[2] `tan_fov` (the capturable entry points)."""
+    return (pi.P, pi.W, pi.H, _ptr(pi.xyz), _ptr(pi.scaling), _ptr(pi.rotation), _ptr(pi.dirs), _ptr(pi.f_dc), _ptr(pi.f_rest),
+            _ptr(pi.opacity), _ptr(pi.label), _ptr(pi.conf), _ptr(pi.V), _ptr(pi.Pm), _ptr(pi.campos),
+            _ptr(_f32(tan_fov, "tan_fov", pi.device)), pi.mod, pi.sh_degree, pi.flags, pi.det_eps)
+
+
 def alloc_outputs(P: int, dev: torch.device, want_cov3D: bool = False, means2D_out: Optional[torch.Tensor] = None):
     f32 = torch.float32
     return {"means2D": means2D_out if means2D_out is not None else empty_rows(P, (3,), f32, dev),
@@ -148,6 +155,29 @@ def project_forward_binned(pi: ProjectionInputs, means2D_out: Optional[torch.Ten
         return out, radii, geom, img, R, int(max_len.value)
     _C.binning_record(key, R)
     return out, radii, geom, img, R, int(max_len.value), (buf if emitted.value else None)
+
+
+def project_forward_binned_capturable(pi: ProjectionInputs, tan_fov: torch.Tensor, binning: torch.Tensor, capacity: int,
+                                      status: torch.Tensor, num_rendered: Optional[torch.Tensor] = None,
+                                      means2D_out: Optional[torch.Tensor] = None):
+    """gh_project_forward_binned_capturable: project_forward_binned with tan(fov / 2) from the device (2,) tensor
+    `tan_fov`, emit into the caller's `binning` buffer of `capacity` records (_C.binning_workspace) and R left on the
+    device (written to the int32 (1,) `num_rendered` when given).  R > capacity sets bit 0 of the int32 (1,) `status`
+    and renders an empty frame (include/gh_rasterizer.h).  -> (out dict as project_forward, radii, geomBuffer,
+    imgBuffer); continue with `_C.forward_render_capturable`.  No host synchronisation."""
+    from . import _C
+    lib = _capi.load()
+    dev, P = pi.device, pi.P
+    if P == 0:
+        raise RuntimeError("project_forward_binned_capturable: empty model")
+    out = alloc_outputs(P, dev, False, means2D_out)
+    geom, img, radii = _C.alloc_forward_workspaces(P, int(pi.W), int(pi.H), dev)
+    with torch.cuda.device(dev):
+        _capi.check(lib.gh_project_forward_binned_capturable(
+            *_common_args_capturable(pi, tan_fov), _ptr(out["means2D"]), _ptr(out["colors"]), _ptr(out["opacity"]),
+            _ptr(out["conic"]), _ptr(out["visible"]), _ptr(radii), _ptr(geom), _ptr(img), _ptr(binning), int(capacity),
+            _ptr(status), _ptr(num_rendered), 0, _stream(dev)))
+    return out, radii, geom, img
 
 
 _CAM_WS: Dict[tuple, torch.Tensor] = {}
@@ -208,12 +238,14 @@ def set_gradient_arena(storage):
 
 def project_backward(pi: ProjectionInputs, visible: torch.Tensor, geom_buffer: Optional[torch.Tensor] = None,
                      dL_dmeans2D=None, dL_dconic4=None, dL_dcolors=None, dL_dopacity=None,
-                     camera_grads: bool = True, want_means2D_grad: bool = False, nan_flag: Optional[torch.Tensor] = None):
+                     camera_grads: bool = True, want_means2D_grad: bool = False, nan_flag: Optional[torch.Tensor] = None,
+                     tan_fov: Optional[torch.Tensor] = None):
     """Incoming gradients: either the rasterizer's geometry workspace after `gh_backward` (its accumulation records are
     read directly) or the four API-shaped tensors (dL_dmeans2D (P,3), dL_dconic (P,2,2) native layout, dL_dcolors
     (P,10), dL_dopacity (P,1)).  -> dict of parameter gradients (+ 'viewmatrix' (4,4), 'projmatrix' (4,4), 'campos' (3),
     'tanfov' (2) when `camera_grads`, + 'means2D' (P,3) = the incoming NDC gradient when `want_means2D_grad`).
-    `nan_flag` (device int32[1], zeroed by the caller): OR-ed with 1 when a parameter gradient is NaN."""
+    `nan_flag` (device int32[1], zeroed by the caller): OR-ed with 1 when a parameter gradient is NaN.
+    `tan_fov`: tan(fov / 2) as a device (2,) tensor instead of the floats in `pi` (gh_project_backward_capturable)."""
     lib = _capi.load()
     dev, P = pi.device, pi.P
     f = dict(dtype=torch.float32, device=dev)
@@ -235,13 +267,15 @@ def project_backward(pi: ProjectionInputs, visible: torch.Tensor, geom_buffer: O
         with torch.cuda.device(dev):
             ws = _camera_workspace(P, dev) if camera_grads else None
             conic4 = _f32(dL_dconic4, "dL_dconic", dev, align=16)
-            _capi.check(lib.gh_project_backward(
-                *_common_args(pi), _ptr(visible), _ptr(geom_buffer),
-                _ptr(_f32(dL_dmeans2D, "dL_dmeans2D", dev)), _ptr(conic4), _ptr(_f32(dL_dcolors, "dL_dcolors", dev, align=8)),
-                _ptr(_f32(dL_dopacity, "dL_dopacity", dev)),
-                _ptr(g["xyz"]), _ptr(g["scaling"]), _ptr(g["rotation"]), _ptr(g["dirs"]), _ptr(g["f_dc"]), _ptr(g["f_rest"]),
-                _ptr(g["opacity"]), _ptr(g["label"]), _ptr(g["conf"]), _ptr(g["means2D"]), _ptr(cam), _ptr(nan_flag), _ptr(ws),
-                _stream(dev)))
+            args = (_ptr(visible), _ptr(geom_buffer),
+                    _ptr(_f32(dL_dmeans2D, "dL_dmeans2D", dev)), _ptr(conic4), _ptr(_f32(dL_dcolors, "dL_dcolors", dev, align=8)),
+                    _ptr(_f32(dL_dopacity, "dL_dopacity", dev)),
+                    _ptr(g["xyz"]), _ptr(g["scaling"]), _ptr(g["rotation"]), _ptr(g["dirs"]), _ptr(g["f_dc"]), _ptr(g["f_rest"]),
+                    _ptr(g["opacity"]), _ptr(g["label"]), _ptr(g["conf"]), _ptr(g["means2D"]), _ptr(cam), _ptr(nan_flag), _ptr(ws))
+            if tan_fov is None:
+                _capi.check(lib.gh_project_backward(*_common_args(pi), *args, _stream(dev)))
+            else:
+                _capi.check(lib.gh_project_backward_capturable(*_common_args_capturable(pi, tan_fov), *args, 0, _stream(dev)))
     if camera_grads:
         g["viewmatrix"], g["projmatrix"] = cam[0:16].view(4, 4), cam[16:32].view(4, 4)
         g["campos"], g["tanfov"] = cam[32:35], cam[35:37]

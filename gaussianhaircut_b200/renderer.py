@@ -26,7 +26,7 @@ import torch.nn.functional as F
 from . import _C, projection
 from ._alloc import empty_rows
 
-__all__ = ["render", "render_hair", "render_hair_strands", "render_raw", "set_nan_flag"]
+__all__ = ["render", "render_hair", "render_hair_strands", "render_raw", "render_raw_capturable", "set_nan_flag"]
 
 _EMPTY = torch.Tensor([])
 
@@ -165,6 +165,64 @@ class _FusedRender(torch.autograd.Function):
         return (pick("xyz", 0), pick("scaling", 1), pick("rotation", 2), pick("dirs", 3), pick("f_dc", 4), pick("f_rest", 5),
                 pick("opacity", 6), pick("label", 7), pick("conf", 8), g_view if need[9] else None,
                 pick("viewmatrix", 10), pick("projmatrix", 11), pick("campos", 12), pick("tanfov", 13), None)
+
+
+class _CapturableRender(torch.autograd.Function):
+    """The capturable twin of _FusedRender's fused path (n_head == 0, GaussianModel rows): (xyz, scaling, rotation, f_dc,
+    f_rest, opacity, label, conf, viewspace, viewmatrix, projmatrix, campos, tan_fov, static) -> (raw image, radii), with
+    the same gradients.  The camera tensors are static device inputs (no camera gradients) and R never leaves the device:
+    `static` holds the caller's binning buffer, its capacity and the status word (render_raw_capturable)."""
+
+    @staticmethod
+    def forward(ctx, xyz, scaling, rotation, f_dc, f_rest, opacity, label, conf, viewspace, viewmatrix, projmatrix, campos,
+                tan_fov, static):
+        st = static
+        # (tan fov is read from `tan_fov` on the device: the host floats of pack_inputs are unused placeholders)
+        pi = projection.pack_inputs(xyz, scaling, rotation, None, f_dc, f_rest, opacity, label, conf, viewmatrix, projmatrix,
+                                    campos, 0.0, 0.0, st["W"], st["H"], st["sh_degree"], st["mod"], st["cfg"])
+        out, radii, geom, img = projection.project_forward_binned_capturable(
+            pi, tan_fov, st["binning"], st["capacity"], st["status"], st["num_rendered"], means2D_out=viewspace.detach())
+        color = _C.forward_render_capturable(st["bg"], out["colors"], geom, st["binning"], img, st["capacity"], st["H"], st["W"])
+        ctx.pi, ctx.st, ctx.tan_fov = pi, st, tan_fov
+        ctx.bufs = (out["colors"], out["visible"], radii, geom, img)
+        ctx.mark_non_differentiable(radii)
+        return color, radii
+
+    @staticmethod
+    def backward(ctx, g_color, _g_radii):
+        pi, st = ctx.pi, ctx.st
+        colors, visible, radii, geom, img = ctx.bufs
+        _C.backward_records_capturable(st["bg"], colors, radii, geom, st["binning"], img, st["capacity"], g_color)
+        g = projection.project_backward(pi, visible, geom_buffer=geom, camera_grads=False, want_means2D_grad=True,
+                                        nan_flag=_NAN_FLAG["t"], tan_fov=ctx.tan_fov)
+        need = ctx.needs_input_grad
+        pick = lambda k, idx: g.get(k) if need[idx] else None  # noqa: E731
+        return (pick("xyz", 0), pick("scaling", 1), pick("rotation", 2), pick("f_dc", 3), pick("f_rest", 4),
+                pick("opacity", 5), pick("label", 6), pick("conf", 7), g["means2D"] if need[8] else None,
+                None, None, None, None, None)
+
+
+def render_raw_capturable(camera: Dict[str, torch.Tensor], pc, bg_color: torch.Tensor, width: int, height: int,
+                          binning: torch.Tensor, capacity: int, status: torch.Tensor,
+                          num_rendered: Optional[torch.Tensor] = None, scaling_modifier: float = 1.0):
+    """`render_raw` for CUDA-graph capture (graphs.CapturedTrainStep): no host synchronisation, and every value that
+    changes between iterations is read on the device.  `camera`: device float32 tensors "viewmatrix" (4,4),
+    "projmatrix" (4,4), "campos" (3) and "tan_fov" (2) = tan(FoV / 2) (x, y), none of which may require grad.
+    `binning`: a buffer of `capacity` records (_C.binning_workspace); `status`: int32 (1,), zeroed by the caller,
+    receives bit 0 when R exceeds the capacity -- the frame then renders as the background, with zero radii and zero
+    gradients; `num_rendered`: int32 (1,) that receives R, or None.  -> (raw (10,H,W) image, radii, viewspace_points)."""
+    for k in ("viewmatrix", "projmatrix", "campos", "tan_fov"):
+        if camera[k].requires_grad:
+            raise RuntimeError(f"render_raw_capturable: camera tensor '{k}' requires grad; trainable cameras are not supported")
+    P = int(pc._xyz.shape[0])
+    viewspace = empty_rows(P, (3,), torch.float32, pc._xyz.device).requires_grad_(True)
+    st = {"W": int(width), "H": int(height), "bg": bg_color, "mod": float(scaling_modifier), "sh_degree": int(pc.active_sh_degree),
+          "cfg": projection.GAUSSIAN_MODEL, "binning": binning, "capacity": int(capacity), "status": status,
+          "num_rendered": num_rendered}
+    renders, radii = _CapturableRender.apply(
+        pc._xyz, pc._scaling, pc._rotation, pc._features_dc, pc._features_rest, pc._opacity, pc._label, pc._orient_conf,
+        viewspace, camera["viewmatrix"], camera["projmatrix"], camera["campos"], camera["tan_fov"], st)
+    return renders, radii, viewspace
 
 
 def _post(renders: torch.Tensor, radii: torch.Tensor, viewspace: torch.Tensor) -> Dict[str, torch.Tensor]:

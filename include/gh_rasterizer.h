@@ -341,6 +341,78 @@ int gh_project_backward(
     unsigned int* nan_flag, void* workspace, gh_stream_t stream);
 
 /*
+ * Capturable training iteration (CUDA graphs; DESIGN §16).  These entry points do the work of the calls they are named
+ * after for the GaussianModel call shape (fused projection, conic supplied, records mode), but none of them
+ * synchronises with the host, allocates, or takes a value that changes between iterations as a host argument, so a
+ * stream capture of them can be replayed for every camera and every step:
+ *   - tan(fov / 2) is read from `tan_fov`, a device float[2] (x, y);
+ *   - R, the number of tile instances, and the longest tile list exist only on the device;
+ *   - the binning buffer holds `capacity` records (gh_binning_workspace_size(capacity) bytes), the deterministic
+ *     workspace gh_backward_det_workspace_size(P, capacity) bytes; capacity lies in [0, 2^32).
+ * Overflow (R > capacity) is safe by construction: the first phase ORs GH_STATUS_BINNING_OVERFLOW into the caller's
+ * device uint32 `status` and empties the frame -- every radius 0, every tile range (0, 0) -- so that no kernel reads
+ * or writes a binning record at or beyond `capacity`, and every output is still written: the image is the background
+ * (final_T = 1, n_contrib = 0), the accumulation records and all gradients are zero.  Pass `status` as the skip_flag
+ * of gh_adam_step_capturable so that the iteration's update is skipped on the device, and zero it before each
+ * iteration.  Each entry point rejects debug != 0, and any call while the stage timer is on, with GH_E_INVALID_ARG
+ * before it launches anything.
+ *
+ * gh_project_forward_binned_capturable: gh_project_forward_binned (non-strand flags; no cov3D) with tan fov from the
+ *   device, no read-back and no pinned memory; emit is always enqueued into `binning_buffer`.  num_rendered (device
+ *   uint32, or NULL) receives R, also on overflow.  `status` is required.
+ * gh_forward_render_capturable: per-tile sort and blend of gh_forward_render (emitted = 1) with R and the longest list
+ *   taken on the device: the long-list split and segment sort are always launched, on grids bounded by T and
+ *   `capacity`, and their CTAs leave at once when no list exceeds the in-kernel sort's 1792 records.  With the same
+ *   inputs and R <= capacity the image, final_T, n_contrib and the sorted lists are bit-identical to gh_forward_render.
+ * gh_backward_capturable: the records-mode blend backward of gh_backward (conic supplied, the four 2-D gradient
+ *   outputs NULL): the accumulation records are left in the geometry workspace.  det_buffer selects the deterministic
+ *   variant as in gh_backward (records bit-identical to it); NULL the fast one.  An empty or overflowed frame yields
+ *   zero records (no host branch on R).
+ * gh_project_backward_capturable: gh_project_backward with tan fov from the device.
+ * gh_adam_step_capturable: gh_adam_step with `lrs` a DEVICE float[n_groups] and the device step count `step_state`
+ *   mandatory; same arithmetic, so the same inputs give bit-identical parameters and moments.
+ */
+#define GH_STATUS_BINNING_OVERFLOW 1u
+int gh_project_forward_binned_capturable(
+    int P, int width, int height,
+    const float* xyz, const float* scaling, const float* rotation, const float* dirs,
+    const float* features_dc, const float* features_rest,
+    const float* opacity, const float* label, const float* orient_conf,
+    const float* viewmatrix, const float* projmatrix, const float* campos,
+    const float* tan_fov, float scale_modifier, int sh_degree, unsigned int flags, float det_eps,
+    float* means2D, float* colors, float* opacities, float* conic, unsigned char* visible,
+    int* radii, char* geom_buffer, char* img_buffer, char* binning_buffer, long long capacity,
+    unsigned int* status, unsigned int* num_rendered, int debug, gh_stream_t stream);
+int gh_forward_render_capturable(
+    int P, int width, int height, long long capacity,
+    const float* background, const float* colors_precomp,
+    char* geom_buffer, char* binning_buffer, char* img_buffer,
+    float* out_color, int debug, gh_stream_t stream);
+int gh_backward_capturable(
+    int P, int width, int height, long long capacity,
+    const float* background, const float* colors_precomp, const int* radii,
+    char* geom_buffer, char* binning_buffer, char* img_buffer,
+    const float* dL_dpix, int debug, gh_stream_t stream, char* det_buffer, size_t det_bytes);
+int gh_project_backward_capturable(
+    int P, int width, int height,
+    const float* xyz, const float* scaling, const float* rotation, const float* dirs,
+    const float* features_dc, const float* features_rest,
+    const float* opacity, const float* label, const float* orient_conf,
+    const float* viewmatrix, const float* projmatrix, const float* campos,
+    const float* tan_fov, float scale_modifier, int sh_degree, unsigned int flags, float det_eps,
+    const unsigned char* visible,
+    const char* geom_buffer,
+    const float* dL_dmeans2D, const float* dL_dconic, const float* dL_dcolors, const float* dL_dopacity,
+    float* d_xyz, float* d_scaling, float* d_rotation, float* d_dirs, float* d_features_dc, float* d_features_rest,
+    float* d_opacity, float* d_label, float* d_orient_conf, float* d_means2D, float* d_camera,
+    unsigned int* nan_flag, void* workspace, int debug, gh_stream_t stream);
+int gh_adam_step_capturable(int n_groups, float* const* params, const float* const* grads,
+                            float* const* exp_avg, float* const* exp_avg_sq,
+                            const unsigned long long* sizes, const float* lrs,
+                            float beta1, float beta2, float eps, int* step_state,
+                            unsigned int* nan_flag, const unsigned int* skip_flag, int debug, gh_stream_t stream);
+
+/*
  * Strand geometry (src/scene/gaussian_model_strands.py:435-454) for the strand mode of the projection (flag bit 10).
  * S strands of L segments, strand-major rows; device float32, contiguous.
  * gh_strand_midpoints: origins (S,1,3), dirs (S,L,3) segment vectors -> xyz (S*L,3) segment midpoints

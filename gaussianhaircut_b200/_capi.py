@@ -127,6 +127,9 @@ SIGNATURES = {
     "gh_orient_workspace_size": (_i, [_i, _i, _i, _i, _i, C.POINTER(_sz)]),   # H W N K num_filters bytes
     "gh_orient_dog": (_i, [_i, _i, _i, _p, _p, _i, _p, _i, _p, _p, _sz, _p]),  # H W C image w_low r_low w_high r_high dog ws bytes stream
     "gh_orient_gabor": (_i, [_i, _i, _p, _i, _i, _i, _p, _p, _p, _p, _sz, _p]),  # H W bank N K nf thetas orients var ws bytes stream
+    "gh_camera_forward": (_i, [_i, _p, _p, _p, _p, _p, _p, _p, _p, _i, _p]),   # n residuals base index view proj campos tan status debug stream
+    "gh_camera_backward": (_i, [_i, _p, _p, _p, _i, _p, _p, _p, _p, _p, _i, _p]),   # n residuals base index intrinsics d_camera grad touched nan status debug stream
+    "gh_camera_adam_step": (_i, [_i, _i, _p, _p, _p, _p, _p, _p, _p, _f, _f, _f, _p, _p, _i, _p]),   # n intrinsics r grad touched m v steps lrs b1 b2 eps nan skip debug stream
 }
 
 _lib = None

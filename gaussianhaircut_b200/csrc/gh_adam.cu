@@ -5,6 +5,7 @@
 // done there with seven blocking `.isnan().any()` host syncs) is a device-side flag: no host sync.
 #include "gh_common.cuh"
 #include "gh_kernels.h"
+#include "gh_adam_math.cuh"
 #include "../../include/gh_rasterizer.h"
 
 namespace {
@@ -18,21 +19,6 @@ struct GhAdamGroups {
     float lr[GH_ADAM_MAX_GROUPS];
     int n;
 };
-
-// MUFU-based square root / reciprocal (about 1 ulp each): the update is bandwidth bound only if the
-// per-element arithmetic stays short.  The result differs from torch's IEEE sqrt + divide by a few
-// ulp of the UPDATE, i.e. ~1e-7 * lr relative to the parameter.
-__device__ __forceinline__ float gh_sqrt_approx(float x) { float r; asm("sqrt.approx.f32 %0, %1;" : "=f"(r) : "f"(x)); return r; }
-__device__ __forceinline__ float gh_rcp_approx(float x) { float r; asm("rcp.approx.f32 %0, %1;" : "=f"(r) : "f"(x)); return r; }
-
-struct GhAdamConst { float beta1, beta2, omb1, omb2, eps, inv_bc2s, step_size; };
-
-__device__ __forceinline__ void gh_adam_elem(float& p, float gr, float& m, float& v, const GhAdamConst& c) {
-    m = fmaf(c.omb1, gr - m, m);                           // exp_avg.lerp_(grad, 1 - beta1)
-    v = fmaf(v, c.beta2, (c.omb2 * gr) * gr);              // mul_(beta2).addcmul_(grad, grad, 1 - beta2)
-    const float denom = fmaf(gh_sqrt_approx(v), c.inv_bc2s, c.eps);   // sqrt(v) / sqrt(bias_correction2) + eps
-    p = fmaf(-(c.step_size * m), gh_rcp_approx(denom), p);            // addcdiv_(exp_avg, denom, -lr / bias_correction1)
-}
 
 // grid = (blocks, groups): blockIdx.y is the parameter group, float4 per thread when the group's four
 // arrays are 16-byte aligned (torch allocations are), scalar tail / fallback otherwise.
@@ -71,8 +57,8 @@ gh_adam_update_body(const GhAdamGroups& g, const float* __restrict__ lr_dev, flo
     if (step_state != nullptr) {
         // device-resident step count (only advanced by steps that were not skipped, like torch's state['step'])
         const int step = step_state[0] + 1;
-        bc1 = 1.0f - powf(beta1, (float)step);
-        bc2_sqrt = sqrtf(1.0f - powf(beta2, (float)step));
+        bc1 = gh_adam_bc1(beta1, step);
+        bc2_sqrt = gh_adam_bc2_sqrt(beta2, step);
     }
     const int k = blockIdx.y;
     const unsigned long long n = g.end[k] - (k ? g.end[k - 1] : 0ull);
@@ -80,9 +66,7 @@ gh_adam_update_body(const GhAdamGroups& g, const float* __restrict__ lr_dev, flo
     const float* __restrict__ G = g.grad[k];
     float* __restrict__ M = g.exp_avg[k];
     float* __restrict__ V = g.exp_avg_sq[k];
-    GhAdamConst c;
-    c.beta1 = beta1; c.beta2 = beta2; c.omb1 = 1.0f - beta1; c.omb2 = 1.0f - beta2; c.eps = eps;
-    c.inv_bc2s = 1.0f / bc2_sqrt; c.step_size = (DEV_LR ? lr_dev[k] : g.lr[k]) / bc1;
+    const GhAdamConst c = gh_adam_const(beta1, beta2, eps, DEV_LR ? lr_dev[k] : g.lr[k], bc1, bc2_sqrt);
     const unsigned long long tid = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
     const unsigned long long nthreads = (unsigned long long)gridDim.x * blockDim.x;
     unsigned long long done = 0;

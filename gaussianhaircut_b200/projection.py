@@ -239,13 +239,14 @@ def set_gradient_arena(storage):
 def project_backward(pi: ProjectionInputs, visible: torch.Tensor, geom_buffer: Optional[torch.Tensor] = None,
                      dL_dmeans2D=None, dL_dconic4=None, dL_dcolors=None, dL_dopacity=None,
                      camera_grads: bool = True, want_means2D_grad: bool = False, nan_flag: Optional[torch.Tensor] = None,
-                     tan_fov: Optional[torch.Tensor] = None):
+                     tan_fov: Optional[torch.Tensor] = None, d_camera: Optional[torch.Tensor] = None):
     """Incoming gradients: either the rasterizer's geometry workspace after `gh_backward` (its accumulation records are
     read directly) or the four API-shaped tensors (dL_dmeans2D (P,3), dL_dconic (P,2,2) native layout, dL_dcolors
     (P,10), dL_dopacity (P,1)).  -> dict of parameter gradients (+ 'viewmatrix' (4,4), 'projmatrix' (4,4), 'campos' (3),
     'tanfov' (2) when `camera_grads`, + 'means2D' (P,3) = the incoming NDC gradient when `want_means2D_grad`).
     `nan_flag` (device int32[1], zeroed by the caller): OR-ed with 1 when a parameter gradient is NaN.
-    `tan_fov`: tan(fov / 2) as a device (2,) tensor instead of the floats in `pi` (gh_project_backward_capturable)."""
+    `tan_fov`: tan(fov / 2) as a device (2,) tensor instead of the floats in `pi` (gh_project_backward_capturable).
+    `d_camera`: with `camera_grads`, a caller-owned contiguous float32 (37,) buffer for the camera gradients."""
     lib = _capi.load()
     dev, P = pi.device, pi.P
     f = dict(dtype=torch.float32, device=dev)
@@ -262,7 +263,11 @@ def project_backward(pi: ProjectionInputs, visible: torch.Tensor, geom_buffer: O
     g = {k: views[k] if has.get(k, True) else None for k, _, _ in GRAD_SEGMENTS}
     del views
     g["means2D"] = empty_rows(P, (3,), torch.float32, dev) if want_means2D_grad else None
-    cam = torch.zeros(37, **f) if camera_grads else None
+    cam = None
+    if camera_grads:
+        cam = torch.zeros(37, **f) if d_camera is None else d_camera
+        if d_camera is not None and P == 0:
+            cam.zero_()
     if P != 0:
         with torch.cuda.device(dev):
             ws = _camera_workspace(P, dev) if camera_grads else None

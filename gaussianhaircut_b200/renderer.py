@@ -170,8 +170,9 @@ class _FusedRender(torch.autograd.Function):
 class _CapturableRender(torch.autograd.Function):
     """The capturable twin of _FusedRender's fused path (n_head == 0, GaussianModel rows): (xyz, scaling, rotation, f_dc,
     f_rest, opacity, label, conf, viewspace, viewmatrix, projmatrix, campos, tan_fov, static) -> (raw image, radii), with
-    the same gradients.  The camera tensors are static device inputs (no camera gradients) and R never leaves the device:
-    `static` holds the caller's binning buffer, its capacity and the status word (render_raw_capturable)."""
+    the same gradients.  The camera tensors are static device inputs and R never leaves the device: `static` holds the
+    caller's binning buffer, its capacity, the status word and the optional d_camera buffer that receives the camera
+    gradients (render_raw_capturable)."""
 
     @staticmethod
     def forward(ctx, xyz, scaling, rotation, f_dc, f_rest, opacity, label, conf, viewspace, viewmatrix, projmatrix, campos,
@@ -193,8 +194,10 @@ class _CapturableRender(torch.autograd.Function):
         pi, st = ctx.pi, ctx.st
         colors, visible, radii, geom, img = ctx.bufs
         _C.backward_records_capturable(st["bg"], colors, radii, geom, st["binning"], img, st["capacity"], g_color)
-        g = projection.project_backward(pi, visible, geom_buffer=geom, camera_grads=False, want_means2D_grad=True,
-                                        nan_flag=_NAN_FLAG["t"], tan_fov=ctx.tan_fov)
+        d_camera = st.get("d_camera")
+        g = projection.project_backward(pi, visible, geom_buffer=geom, camera_grads=d_camera is not None,
+                                        want_means2D_grad=True, nan_flag=_NAN_FLAG["t"], tan_fov=ctx.tan_fov,
+                                        d_camera=d_camera)
         need = ctx.needs_input_grad
         pick = lambda k, idx: g.get(k) if need[idx] else None  # noqa: E731
         return (pick("xyz", 0), pick("scaling", 1), pick("rotation", 2), pick("f_dc", 3), pick("f_rest", 4),
@@ -204,13 +207,17 @@ class _CapturableRender(torch.autograd.Function):
 
 def render_raw_capturable(camera: Dict[str, torch.Tensor], pc, bg_color: torch.Tensor, width: int, height: int,
                           binning: torch.Tensor, capacity: int, status: torch.Tensor,
-                          num_rendered: Optional[torch.Tensor] = None, scaling_modifier: float = 1.0):
+                          num_rendered: Optional[torch.Tensor] = None, scaling_modifier: float = 1.0,
+                          d_camera: Optional[torch.Tensor] = None):
     """`render_raw` for CUDA-graph capture (graphs.CapturedTrainStep): no host synchronisation, and every value that
     changes between iterations is read on the device.  `camera`: device float32 tensors "viewmatrix" (4,4),
     "projmatrix" (4,4), "campos" (3) and "tan_fov" (2) = tan(FoV / 2) (x, y), none of which may require grad.
     `binning`: a buffer of `capacity` records (_C.binning_workspace); `status`: int32 (1,), zeroed by the caller,
     receives bit 0 when R exceeds the capacity -- the frame then renders as the background, with zero radii and zero
-    gradients; `num_rendered`: int32 (1,) that receives R, or None.  -> (raw (10,H,W) image, radii, viewspace_points)."""
+    gradients; `num_rendered`: int32 (1,) that receives R, or None; `d_camera`: None, or a device float32 (37,) buffer
+    that the backward fills with the camera gradients in gh_project_backward's d_camera layout (dL/dviewmatrix,
+    dL/dprojmatrix, dL/dcampos, dL/dtan_fov) -- the input of cameras.CameraRig.backward.
+    -> (raw (10,H,W) image, radii, viewspace_points)."""
     for k in ("viewmatrix", "projmatrix", "campos", "tan_fov"):
         if camera[k].requires_grad:
             raise RuntimeError(f"render_raw_capturable: camera tensor '{k}' requires grad; trainable cameras are not supported")
@@ -218,7 +225,7 @@ def render_raw_capturable(camera: Dict[str, torch.Tensor], pc, bg_color: torch.T
     viewspace = empty_rows(P, (3,), torch.float32, pc._xyz.device).requires_grad_(True)
     st = {"W": int(width), "H": int(height), "bg": bg_color, "mod": float(scaling_modifier), "sh_degree": int(pc.active_sh_degree),
           "cfg": projection.GAUSSIAN_MODEL, "binning": binning, "capacity": int(capacity), "status": status,
-          "num_rendered": num_rendered}
+          "num_rendered": num_rendered, "d_camera": d_camera}
     renders, radii = _CapturableRender.apply(
         pc._xyz, pc._scaling, pc._rotation, pc._features_dc, pc._features_rest, pc._opacity, pc._label, pc._orient_conf,
         viewspace, camera["viewmatrix"], camera["projmatrix"], camera["campos"], camera["tan_fov"], st)
@@ -238,13 +245,19 @@ def _post(renders: torch.Tensor, radii: torch.Tensor, viewspace: torch.Tensor) -
 
 
 def _static(viewpoint_camera, bg_color, scaling_modifier, sh_degree, debug, cfg) -> Dict[str, object]:
-    return {"W": int(viewpoint_camera.image_width), "H": int(viewpoint_camera.image_height),
-            "tanx": _tan_half(viewpoint_camera.FoVx), "tany": _tan_half(viewpoint_camera.FoVy),
+    tan = getattr(viewpoint_camera, "tan_fov", None)        # a cameras.CameraRig view: tan(FoV / 2) on the device
+    tanx, tany = (tan.tolist() if tan is not None else
+                  (_tan_half(viewpoint_camera.FoVx), _tan_half(viewpoint_camera.FoVy)))
+    return {"W": int(viewpoint_camera.image_width), "H": int(viewpoint_camera.image_height), "tanx": tanx, "tany": tany,
             "bg": bg_color, "mod": float(scaling_modifier), "sh_degree": int(sh_degree), "debug": bool(debug), "cfg": cfg}
 
 
 def _tanfov_tensor(viewpoint_camera):
-    """A differentiable (2,) tensor when the field of view is trainable (cameras.py:95-107), else None."""
+    """A differentiable (2,) tensor when the field of view is trainable (cameras.py:95-107), else None.  A camera with a
+    `tan_fov` attribute (cameras.CameraRig views) hands that tensor over as it is."""
+    tan = getattr(viewpoint_camera, "tan_fov", None)
+    if tan is not None:
+        return tan
     fx, fy = viewpoint_camera.FoVx, viewpoint_camera.FoVy
     if isinstance(fx, torch.Tensor) and isinstance(fy, torch.Tensor) and (fx.requires_grad or fy.requires_grad):
         return torch.stack([torch.tan(fx * 0.5).reshape(()), torch.tan(fy * 0.5).reshape(())])

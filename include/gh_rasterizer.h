@@ -413,6 +413,49 @@ int gh_adam_step_capturable(int n_groups, float* const* params, const float* con
                             unsigned int* nan_flag, const unsigned int* skip_flag, int debug, gh_stream_t stream);
 
 /*
+ * Trainable cameras (DESIGN §17): the reference's BARF camera model (src/scene/cameras.py:95-152, use_barf = True) and
+ * its camera Adam (src/train_gaussians.py:45-63, 183-196).  A rig of n cameras owns, on the device:
+ *   base       float[n][18]  C = the float32 _colmap_transform (16, row-major), FoVx, FoVy (the camera's base state)
+ *   residuals  float[n][8]   r = [w (3), u (3), f (2)] = _rotation_res, _translation_res, _fov_res (f = 0 without
+ *                            trainable intrinsics)
+ *   grad       float[n][8]   dL/dr, accumulated by gh_camera_backward
+ *   touched    int[n]        1 for a row gh_camera_backward wrote since the last gh_camera_adam_step
+ * with znear = 0.01, zfar = 100:
+ *   viewmatrix = (C @ Res)^T, Res[:3] = lie.se3_to_SE3(cat(w, u)), Res[3] = (0, 0, 0, 1)
+ *   projmatrix = viewmatrix @ getProjectionMatrix(znear, zfar, FoVx + f0, FoVy + f1)^T
+ *   campos     = inverse(viewmatrix)[3, :3],   tan_fov = tan((FoV + f) / 2) per axis (x, y)
+ * (arithmetic: gaussianhaircut_b200/csrc/gh_camera_math.h).  Every entry point reads the camera index from the device
+ * int32 `index`, so a captured CUDA graph serves every view; an index outside [0, n) ORs GH_STATUS_CAMERA_INDEX into
+ * the device uint32 `status` and the kernel touches nothing else.  None of them synchronises with the host.  Each
+ * rejects n <= 0, a missing or misaligned (not 4-byte) pointer, debug != 0 and calls while the stage timer is on with
+ * GH_E_INVALID_ARG before it launches anything.
+ *
+ * gh_camera_forward: the four outputs of camera `index` into viewmatrix (16), projmatrix (16), campos (3), tan_fov (2),
+ *   row-major like the reference's tensors.
+ * gh_camera_backward: d_camera (float[37], the layout of gh_project_backward's d_camera: dL/dviewmatrix, dL/dprojmatrix,
+ *   dL/dcampos, dL/dtan_fov) -> dL/dr of row `index`, ADDED to grad[index]; touched[index] = 1.  `intrinsics` == 0:
+ *   f is not trained and its two gradients are 0.  nan_flag (device uint32) is OR-ed with 1 when one is NaN.
+ * gh_camera_adam_step: torch.optim.Adam (the arithmetic of gh_adam_step_capturable) on exactly the touched rows, each
+ *   with its own step count steps[i]: columns 0-2, 3-5 and 6-7 (the last two only with `intrinsics`) use the device
+ *   learning rates lrs[0] (rotation), lrs[1] (translation), lrs[2] (fov); exp_avg / exp_avg_sq are float[n][8].  The
+ *   touched rows' gradients and marks are then cleared -- torch.optim.Adam after zero_grad(set_to_none=True): a camera
+ *   that was not visited does not step.  When *nan_flag or *skip_flag (device uint32, may be NULL: e.g. the binning
+ *   status word) is non-zero the update is skipped as a whole (moments and step counts unchanged), the gradients are
+ *   still cleared.  *nan_flag is zeroed at the end.
+ */
+#define GH_STATUS_CAMERA_INDEX 2u
+int gh_camera_forward(int n, const float* residuals, const float* base, const int* index,
+                      float* viewmatrix, float* projmatrix, float* campos, float* tan_fov,
+                      unsigned int* status, int debug, gh_stream_t stream);
+int gh_camera_backward(int n, const float* residuals, const float* base, const int* index, int intrinsics,
+                       const float* d_camera, float* grad, int* touched, unsigned int* nan_flag,
+                       unsigned int* status, int debug, gh_stream_t stream);
+int gh_camera_adam_step(int n, int intrinsics, float* residuals, float* grad, int* touched,
+                        float* exp_avg, float* exp_avg_sq, int* steps, const float* lrs,
+                        float beta1, float beta2, float eps, unsigned int* nan_flag,
+                        const unsigned int* skip_flag, int debug, gh_stream_t stream);
+
+/*
  * Strand geometry (src/scene/gaussian_model_strands.py:435-454) for the strand mode of the projection (flag bit 10).
  * S strands of L segments, strand-major rows; device float32, contiguous.
  * gh_strand_midpoints: origins (S,1,3), dirs (S,L,3) segment vectors -> xyz (S*L,3) segment midpoints

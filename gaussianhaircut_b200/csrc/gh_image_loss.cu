@@ -152,27 +152,40 @@ gh_loss_presum_kernel(const float* __restrict__ gt_orient_conf, size_t n, double
 }
 
 // Pointwise terms of one pixel: loss contributions (returned through the accumulators) and dL/dout for
-// channels 3..9.
+// channels 3..9 (and 0..2 in the latent-strand stage, which has no SSIM pass).
+//   STAGE 0 (appearance):     L1 masked by gt_mask[1]; mask L1 over both channels
+//   STAGE 1 (strands):        L1 unmasked (m1 = 1, exact); mask L1 over both channels
+//   STAGE 2 (latent strands): L1 unmasked, its gradient written here; mask L1 over channel 3 only, channel 4 zero
+//   OPTS: GH_LOSS_ORIENT_UNIT_WEIGHT (w = 1, sum of weights = W H), GH_LOSS_ORIENT_NO_CONF (no confidence factor and
+//   no log term: channel 8 is zero)
+template <int STAGE, unsigned OPTS>
 __device__ __forceinline__ void gh_loss_pointwise(const GhLossParams& prm, size_t plane, size_t pi, float inv_sum_w,
                                                   const float* __restrict__ out, const float* __restrict__ gt_image,
                                                   const float* __restrict__ gt_mask, const float* __restrict__ gt_angle,
                                                   const float* __restrict__ gt_conf, float* __restrict__ dL,
                                                   double& a_l1, double& a_mask, double& a_orient)
 {
-    const float m0 = gt_mask[pi], m1 = gt_mask[plane + pi];
-    // masked L1 on the image (value only; its gradient is written with the SSIM gradient)
+    constexpr bool unit_w = (OPTS & GH_LOSS_ORIENT_UNIT_WEIGHT) != 0, no_conf = (OPTS & GH_LOSS_ORIENT_NO_CONF) != 0;
+    const float m0 = gt_mask[pi], m1 = (STAGE == 0) ? gt_mask[plane + pi] : 1.f;
+    // masked L1 on the image (value only; its gradient is written with the SSIM gradient, or here in stage 2)
+    const float s_l1 = prm.l_dl1 / (float)(3.0 * (double)plane);
 #pragma unroll
-    for (int c = 0; c < 3; c++) a_l1 += (double)(fabsf(out[c * plane + pi] - gt_image[c * plane + pi]) * m1);
-    // L1 on the two mask channels
-    const float dm_scale = prm.l_dmask / (float)(2.0 * (double)plane);
+    for (int c = 0; c < 3; c++) {
+        a_l1 += (double)(fabsf(out[c * plane + pi] - gt_image[c * plane + pi]) * m1);
+        if constexpr (STAGE == 2) dL[c * plane + pi] = s_l1 * gh_sign(out[c * plane + pi] - gt_image[c * plane + pi]);
+    }
+    // L1 on the two mask channels (stage 2: on channel 3 only)
+    constexpr int NMASK = (STAGE == 2) ? 1 : 2;
+    const float dm_scale = prm.l_dmask / (float)((STAGE == 2 ? 1.0 : 2.0) * (double)plane);
 #pragma unroll
-    for (int k = 0; k < 2; k++) {
+    for (int k = 0; k < NMASK; k++) {
         const float d = out[(3 + k) * plane + pi] - gt_mask[k * plane + pi];
         a_mask += (double)fabsf(d);
         dL[(3 + k) * plane + pi] = dm_scale * gh_sign(d);
     }
+    if constexpr (STAGE == 2) dL[4 * plane + pi] = 0.f;
     // orientation: dir = normalize(out[5:7]), mirrored so that dir.x >= 0, angle = acos(dir.y)/pi
-    const float c5 = out[5 * plane + pi], c6 = out[6 * plane + pi], conf = out[8 * plane + pi];
+    const float c5 = out[5 * plane + pi], c6 = out[6 * plane + pi], conf = no_conf ? 1.f : out[8 * plane + pi];
     const float nrm = sqrtf(c5 * c5 + c6 * c6);
     const float den = fmaxf(nrm, 1e-12f);                  // F.normalize eps
     const float dirx = c5 / den, diry = c6 / den;
@@ -187,16 +200,17 @@ __device__ __forceinline__ void gh_loss_pointwise(const GhLossParams& prm, size_
     const float l0 = fabsf(d0), l1 = fabsf(d1), l2 = fabsf(d2);
     const float inner = fminf(l1, l2);
     const float Lmin = fminf(l0, inner) * PI;
-    const float w = gt_conf[pi];
-    const float lp = (Lmin * conf - logf(conf + 1e-7f)) * m0;
+    const float w = unit_w ? 1.f : gt_conf[pi];
+    const float lp = no_conf ? Lmin * m0 : (Lmin * conf - logf(conf + 1e-7f)) * m0;
     a_orient += (double)(lp * w);
-    // gradients; 1 / sum(w) is known from the presum launch
+    // gradients; 1 / sum(w) is known from the presum launch (W H with unit weights)
     const float up = m0 * w * (prm.l_dorient * inv_sum_w);   // d loss / d (per-pixel loss before mask)
     // torch.minimum splits the gradient evenly on ties
     const float w_outer0 = (l0 < inner) ? 1.f : ((l0 == inner) ? 0.5f : 0.f);
     const float w_in = 1.f - w_outer0;
     const float w1 = (l1 < l2) ? 1.f : ((l1 == l2) ? 0.5f : 0.f);
-    const float dL_dang = up * conf * PI * (w_outer0 * gh_sign(d0) + w_in * (w1 * gh_sign(d1) + (1.f - w1) * gh_sign(d2)));
+    const float upc = no_conf ? up : up * conf;
+    const float dL_dang = upc * PI * (w_outer0 * gh_sign(d0) + w_in * (w1 * gh_sign(d1) + (1.f - w1) * gh_sign(d2)));
     const float dang_dt = -1.f / (PI * sqrtf(fmaxf(1.f - t * t, 0.f)));
     const float dt_ddiry = (diry >= lo && diry <= hi) ? mirror : 0.f;       // clamp passes the gradient inside [lo, hi]
     const float gdy = dL_dang * dang_dt * dt_ddiry;
@@ -211,13 +225,13 @@ __device__ __forceinline__ void gh_loss_pointwise(const GhLossParams& prm, size_
     dL[5 * plane + pi] = gdy * ddy_dc5;
     dL[6 * plane + pi] = gdy * ddy_dc6;
     dL[7 * plane + pi] = 0.f;
-    dL[8 * plane + pi] = up * (Lmin - 1.f / (conf + 1e-7f));
+    dL[8 * plane + pi] = no_conf ? 0.f : up * (Lmin - 1.f / (conf + 1e-7f));
     dL[9 * plane + pi] = 0.f;
 }
 
 // All pointwise terms (masked L1 value, mask L1, orientation) of every pixel: loss sums and dL/dout
-// channels 3..9.  Plain elementwise kernel, one pixel per thread per grid-stride step.
-template <bool DET>
+// channels 3..9 (0..9 in stage 2).  Plain elementwise kernel, one pixel per thread per grid-stride step.
+template <bool DET, int STAGE, unsigned OPTS>
 __global__ void __launch_bounds__(256)
 gh_loss_pointwise_kernel(GhLossParams prm, const float* __restrict__ out, const float* __restrict__ gt_image,
                          const float* __restrict__ gt_mask, const float* __restrict__ gt_angle,
@@ -226,9 +240,10 @@ gh_loss_pointwise_kernel(GhLossParams prm, const float* __restrict__ out, const 
 {
     const size_t plane = (size_t)prm.W * prm.H;
     double a_l1 = 0.0, a_mask = 0.0, a_orient = 0.0;
-    const float inv_sum_w = 1.0f / (float)sums[GH_LS_W];
+    const float inv_sum_w = 1.0f / (float)((OPTS & GH_LOSS_ORIENT_UNIT_WEIGHT) ? (double)plane : sums[GH_LS_W]);
     for (size_t pi = (size_t)blockIdx.x * 256 + threadIdx.x; pi < plane; pi += (size_t)gridDim.x * 256)
-        gh_loss_pointwise(prm, plane, pi, inv_sum_w, out, gt_image, gt_mask, gt_angle, gt_conf, dL, a_l1, a_mask, a_orient);
+        gh_loss_pointwise<STAGE, OPTS>(prm, plane, pi, inv_sum_w, out, gt_image, gt_mask, gt_angle, gt_conf, dL,
+                                       a_l1, a_mask, a_orient);
     if constexpr (DET) {
         double v[3] = {a_l1, a_mask, a_orient};
         gh_block_sum_fixed<3>(v, part, sums, {GH_LS_L1, GH_LS_MASK, GH_LS_ORIENT}, GH_TK_POINTWISE);
@@ -242,8 +257,9 @@ gh_loss_pointwise_kernel(GhLossParams prm, const float* __restrict__ out, const 
 
 // SSIM statistics of a 32x32 tile: separable 11-tap window, register blocked (a thread filters 8
 // adjacent columns of a halo row, then 4 adjacent rows of a column, so a shared-memory value is reused
-// by up to 8 taps) and paired: (x, y) and (x^2, y^2) travel as float2.
-template <int MINB, bool DET>
+// by up to 8 taps) and paired: (x, y) and (x^2, y^2) travel as float2.  STAGE 1 takes the image unmasked (the mask is
+// 1: x * 1 is exact, so this is the STAGE 0 arithmetic without the mask loads).
+template <int MINB, bool DET, int STAGE>
 __global__ void __launch_bounds__(256, MINB)
 gh_loss_main_kernel(GhLossParams prm, const float* __restrict__ out, const float* __restrict__ gt_image,
                     const float* __restrict__ gt_mask, double* __restrict__ sums,
@@ -284,7 +300,7 @@ gh_loss_main_kernel(GhLossParams prm, const float* __restrict__ out, const float
                     const int q = rowbase + (ok ? gx : 0);
                     xo[2 * jj + h] = ok ? oc[q] : 0.f;
                     xg[2 * jj + h] = ok ? gc[q] : 0.f;
-                    xm[2 * jj + h] = ok ? mc[q] : 0.f;                 // zero padding (F.conv2d padding=5)
+                    xm[2 * jj + h] = ok ? (STAGE == 0 ? mc[q] : 1.f) : 0.f;   // zero padding (F.conv2d padding=5)
                 }
             }
 #pragma unroll
@@ -379,7 +395,7 @@ gh_loss_main_kernel(GhLossParams prm, const float* __restrict__ out, const float
     }
 }
 
-template <int MINB>
+template <int MINB, int STAGE>
 __global__ void __launch_bounds__(256, MINB)
 gh_loss_ssim_bwd_kernel(GhLossParams prm, const float* __restrict__ out, const float* __restrict__ gt_image,
                         const float* __restrict__ gt_mask, const float* __restrict__ dmaps, float* __restrict__ dL)
@@ -479,7 +495,7 @@ gh_loss_ssim_bwd_kernel(GhLossParams prm, const float* __restrict__ out, const f
                 const int py = ty0 + 4 * rg + o;
                 if (px < W && py < H) {
                     const int pi = py * W + px;
-                    const float m1 = gt_mask[plane + pi];
+                    const float m1 = (STAGE == 0) ? gt_mask[plane + pi] : 1.f;
                     const float I = out[c * plane + pi], G = gt_image[c * plane + pi];
                     const float x = I * m1, y = G * m1;
                     // the window is symmetric: the adjoint of the convolution is the same convolution
@@ -491,28 +507,135 @@ gh_loss_ssim_bwd_kernel(GhLossParams prm, const float* __restrict__ out, const f
     }
 }
 
-// losses[8]: total, Ll1, Lssim, Lmask, Lorient, sum of orientation weights, Lorient-was-NaN flag, 0
+// losses[8]: total, Ll1, Lssim, Lmask, Lorient, sum of orientation weights, Lorient-was-NaN flag, slot 7.
+// Stage 2 (SRC/train_latent_strands.py:142-152): slot 2 is 0, slot 3 holds LCE, and Ll1, LCE and LOR are each replaced
+// by 0 when NaN, zeroing their gradient channels; slot 7 holds the replaced terms as a bitmask (1 Ll1, 2 LCE).
+template <int STAGE, unsigned OPTS>
 __global__ void __launch_bounds__(256)
 gh_loss_finalize_kernel(GhLossParams prm, const double* __restrict__ sums, float* __restrict__ losses, float* __restrict__ dL)
 {
+    constexpr bool unit_w = (OPTS & GH_LOSS_ORIENT_UNIT_WEIGHT) != 0;
     const size_t plane = (size_t)prm.W * prm.H;
     const double n = (double)plane;
-    const float Lorient_raw = (float)(sums[GH_LS_ORIENT] / sums[GH_LS_W]);
+    const float Lorient_raw = (float)(sums[GH_LS_ORIENT] / (unit_w ? n : sums[GH_LS_W]));
     const bool bad = (Lorient_raw != Lorient_raw);                    // torch.isnan(Lorient).any() -> zeros_like
-    if (blockIdx.x == 0 && threadIdx.x == 0) {
-        const float Ll1 = (float)(sums[GH_LS_L1] / (3.0 * n));
-        const float Lssim = 1.0f - (float)(sums[GH_LS_SSIM] / (3.0 * n));
-        const float Lmask = (float)(sums[GH_LS_MASK] / (2.0 * n));
-        const float Lorient = bad ? 0.f : Lorient_raw;
-        losses[0] = Ll1 * prm.l_dl1 + Lssim * prm.l_dssim + Lmask * prm.l_dmask + Lorient * prm.l_dorient;
-        losses[1] = Ll1; losses[2] = Lssim; losses[3] = Lmask; losses[4] = Lorient;
-        losses[5] = (float)sums[GH_LS_W]; losses[6] = bad ? 1.f : 0.f; losses[7] = 0.f;
+    if constexpr (STAGE == 2) {
+        const float Ll1_raw = (float)(sums[GH_LS_L1] / (3.0 * n));
+        const float LCE_raw = (float)(sums[GH_LS_MASK] / n);
+        const bool bad_l1 = (Ll1_raw != Ll1_raw), bad_ce = (LCE_raw != LCE_raw);
+        if (blockIdx.x == 0 && threadIdx.x == 0) {
+            const float Ll1 = bad_l1 ? 0.f : Ll1_raw, LCE = bad_ce ? 0.f : LCE_raw, LOR = bad ? 0.f : Lorient_raw;
+            losses[0] = Ll1 * prm.l_dl1 + LCE * prm.l_dmask + LOR * prm.l_dorient;
+            losses[1] = Ll1; losses[2] = 0.f; losses[3] = LCE; losses[4] = LOR;
+            losses[5] = (float)(unit_w ? n : sums[GH_LS_W]); losses[6] = bad ? 1.f : 0.f;
+            losses[7] = (bad_l1 ? 1.f : 0.f) + (bad_ce ? 2.f : 0.f);
+        }
+        if (!(bad || bad_l1 || bad_ce)) return;
+        // a replaced term is a constant: nothing flows into its channels
+        for (size_t i = (size_t)blockIdx.x * 256 + threadIdx.x; i < plane; i += (size_t)gridDim.x * 256) {
+            if (bad_l1) { dL[i] = 0.f; dL[plane + i] = 0.f; dL[2 * plane + i] = 0.f; }
+            if (bad_ce) dL[3 * plane + i] = 0.f;
+            if (bad) { dL[5 * plane + i] = 0.f; dL[6 * plane + i] = 0.f; dL[8 * plane + i] = 0.f; }
+        }
+    } else {
+        if (blockIdx.x == 0 && threadIdx.x == 0) {
+            const float Ll1 = (float)(sums[GH_LS_L1] / (3.0 * n));
+            const float Lssim = 1.0f - (float)(sums[GH_LS_SSIM] / (3.0 * n));
+            const float Lmask = (float)(sums[GH_LS_MASK] / (2.0 * n));
+            const float Lorient = bad ? 0.f : Lorient_raw;
+            losses[0] = Ll1 * prm.l_dl1 + Lssim * prm.l_dssim + Lmask * prm.l_dmask + Lorient * prm.l_dorient;
+            losses[1] = Ll1; losses[2] = Lssim; losses[3] = Lmask; losses[4] = Lorient;
+            losses[5] = (float)(unit_w ? n : sums[GH_LS_W]); losses[6] = bad ? 1.f : 0.f; losses[7] = 0.f;
+        }
+        if (!bad) return;
+        // the orientation term was replaced by a constant: nothing flows into channels 5, 6, 8
+        for (size_t i = (size_t)blockIdx.x * 256 + threadIdx.x; i < plane; i += (size_t)gridDim.x * 256) {
+            dL[5 * plane + i] = 0.f; dL[6 * plane + i] = 0.f; dL[8 * plane + i] = 0.f;
+        }
     }
-    if (!bad) return;
-    // the orientation term was replaced by a constant: nothing flows into channels 5, 6, 8
-    for (size_t i = (size_t)blockIdx.x * 256 + threadIdx.x; i < plane; i += (size_t)gridDim.x * 256) {
-        dL[5 * plane + i] = 0.f; dL[6 * plane + i] = 0.f; dL[8 * plane + i] = 0.f;
+}
+
+// The launches of one (stage, options) pair: presum (unless the weights are unit), pointwise, the two SSIM passes
+// (stages 0 and 1), finalize.  Returns the number of kernels launched.
+template <int STAGE, unsigned OPTS>
+int gh_loss_launch(const GhLossParams& prm, const float* out_color, const float* gt_image, const float* gt_mask,
+                   const float* gt_orient_angle, const float* gt_orient_conf, double* sums, float* losses,
+                   float* dL_dout, cudaStream_t stream, bool deterministic)
+{
+    constexpr bool unit_w = (OPTS & GH_LOSS_ORIENT_UNIT_WEIGHT) != 0, ssim = STAGE != 2;
+    const int width = prm.W, height = prm.H;
+    const GhLossParts np = GhLossParts::of(width, height);
+    double* part_presum = sums + GH_LS_COUNT;
+    double* part_pointwise = part_presum + np.rb;
+    double* part_main = part_pointwise + 3 * (size_t)np.pb;
+    float* dmaps = reinterpret_cast<float*>(part_main + np.mb);
+    const size_t plane = (size_t)width * height;
+    const int rb = np.rb, pb = np.pb;
+    const dim3 grid((width + GH_LT - 1) / GH_LT, (height + GH_LT - 1) / GH_LT), block(256);
+    if (deterministic) {
+        if (!unit_w) gh_loss_presum_kernel<true><<<rb, 256, 0, stream>>>(gt_orient_conf, plane, sums, part_presum);
+        gh_loss_pointwise_kernel<true, STAGE, OPTS><<<pb, 256, 0, stream>>>(prm, out_color, gt_image, gt_mask,
+            gt_orient_angle, gt_orient_conf, sums, dL_dout, part_pointwise);
+        if constexpr (ssim)
+            gh_loss_main_kernel<4, true, STAGE><<<grid, block, 0, stream>>>(prm, out_color, gt_image, gt_mask, sums, dmaps, part_main);
+    } else {
+        if (!unit_w) gh_loss_presum_kernel<false><<<rb, 256, 0, stream>>>(gt_orient_conf, plane, sums, nullptr);
+        gh_loss_pointwise_kernel<false, STAGE, OPTS><<<pb, 256, 0, stream>>>(prm, out_color, gt_image, gt_mask,
+            gt_orient_angle, gt_orient_conf, sums, dL_dout, nullptr);
+        // 4 CTAs per SM (64 registers)
+        if constexpr (ssim)
+            gh_loss_main_kernel<4, false, STAGE><<<grid, block, 0, stream>>>(prm, out_color, gt_image, gt_mask, sums, dmaps, nullptr);
     }
+    if constexpr (ssim)
+        gh_loss_ssim_bwd_kernel<4, STAGE><<<grid, block, 0, stream>>>(prm, out_color, gt_image, gt_mask, dmaps, dL_dout);
+    gh_loss_finalize_kernel<STAGE, OPTS><<<rb, 256, 0, stream>>>(prm, sums, losses, dL_dout);
+    return (unit_w ? 0 : 1) + 1 + (ssim ? 2 : 0) + 1;
+}
+
+// Argument checks and launches shared by gh_image_loss and gh_image_loss_stage; `who` names the entry point in the
+// messages.  The stage and option checks are the caller's.
+int gh_image_loss_run(const char* who, int width, int height, int stage, unsigned options, const float* out_color,
+                      const float* gt_image, const float* gt_mask, const float* gt_orient_angle,
+                      const float* gt_orient_conf, float lambda_dl1, float lambda_dssim, float lambda_dmask,
+                      float lambda_dorient, void* workspace, float* losses, float* dL_dout, gh_stream_t stream_,
+                      int deterministic)
+{
+    cudaStream_t stream = (cudaStream_t)stream_;
+    const bool conf_needed = !(options & GH_LOSS_ORIENT_UNIT_WEIGHT);
+    if (width <= 0 || height <= 0 || !out_color || !gt_image || !gt_mask || !gt_orient_angle ||
+        (conf_needed && !gt_orient_conf) || !workspace || !losses || !dL_dout)
+        return gh_set_error(GH_E_INVALID_ARG, "%s: bad size or missing pointer", who);
+    if ((size_t)workspace & 7) return gh_set_error(GH_E_INVALID_ARG, "%s: workspace must be 8-byte aligned", who);
+    if ((long long)width * height > (1ll << 27))      // 32-bit pixel offsets inside the kernels
+        return gh_set_error(GH_E_INVALID_ARG, "%s: image larger than 2^27 pixels", who);
+    GhLossParams prm;
+    prm.W = width; prm.H = height;
+    prm.l_dl1 = lambda_dl1; prm.l_dssim = lambda_dssim; prm.l_dmask = lambda_dmask; prm.l_dorient = lambda_dorient;
+    {   // gaussian(11, 1.5) as the reference builds it: float32 taps, float32 normalisation
+        float g[11], sum = 0.f;
+        for (int k = 0; k < 11; k++) { g[k] = (float)exp(-(double)((k - 5) * (k - 5)) / (2.0 * 1.5 * 1.5)); sum += g[k]; }
+        for (int k = 0; k < 11; k++) prm.g[k] = g[k] / sum;
+    }
+    double* sums = reinterpret_cast<double*>(workspace);
+    const cudaError_t e = cudaMemsetAsync(sums, 0, GH_LS_COUNT * sizeof(double), stream);     // sums + tickets
+    if (e != cudaSuccess) return gh_cuda_status(who, "memset(partial sums)", e);
+    const bool det = deterministic != 0;
+#define GH_LOSS_ARGS prm, out_color, gt_image, gt_mask, gt_orient_angle, gt_orient_conf, sums, losses, dL_dout, stream, det
+    int n = 0;
+    switch (stage * 4 + (int)options) {
+    case 0: n = gh_loss_launch<0, 0u>(GH_LOSS_ARGS); break;
+    case 4: n = gh_loss_launch<1, 0u>(GH_LOSS_ARGS); break;
+    case 5: n = gh_loss_launch<1, 1u>(GH_LOSS_ARGS); break;
+    case 6: n = gh_loss_launch<1, 2u>(GH_LOSS_ARGS); break;
+    case 7: n = gh_loss_launch<1, 3u>(GH_LOSS_ARGS); break;
+    case 8: n = gh_loss_launch<2, 0u>(GH_LOSS_ARGS); break;
+    case 9: n = gh_loss_launch<2, 1u>(GH_LOSS_ARGS); break;
+    case 10: n = gh_loss_launch<2, 2u>(GH_LOSS_ARGS); break;
+    case 11: n = gh_loss_launch<2, 3u>(GH_LOSS_ARGS); break;
+    default: return gh_set_error(GH_E_INVALID_ARG, "%s: unsupported stage %d with options %u", who, stage, options);
+    }
+#undef GH_LOSS_ARGS
+    return gh_launch_status(who, n);
 }
 
 }  // namespace
@@ -530,46 +653,30 @@ extern "C" int gh_image_loss(int width, int height, const float* out_color, cons
                              float lambda_dl1, float lambda_dssim, float lambda_dmask, float lambda_dorient,
                              void* workspace, float* losses, float* dL_dout, gh_stream_t stream_, int deterministic)
 {
-    cudaStream_t stream = (cudaStream_t)stream_;
     gh_clear_error();
-    if (width <= 0 || height <= 0 || !out_color || !gt_image || !gt_mask || !gt_orient_angle || !gt_orient_conf ||
-        !workspace || !losses || !dL_dout)
-        return gh_set_error(GH_E_INVALID_ARG, "gh_image_loss: bad size or missing pointer");
-    if ((size_t)workspace & 7) return gh_set_error(GH_E_INVALID_ARG, "gh_image_loss: workspace must be 8-byte aligned");
-    if ((long long)width * height > (1ll << 27))      // 32-bit pixel offsets inside the kernels
-        return gh_set_error(GH_E_INVALID_ARG, "gh_image_loss: image larger than 2^27 pixels");
-    GhLossParams prm;
-    prm.W = width; prm.H = height;
-    prm.l_dl1 = lambda_dl1; prm.l_dssim = lambda_dssim; prm.l_dmask = lambda_dmask; prm.l_dorient = lambda_dorient;
-    {   // gaussian(11, 1.5) as the reference builds it: float32 taps, float32 normalisation
-        float g[11], sum = 0.f;
-        for (int k = 0; k < 11; k++) { g[k] = (float)exp(-(double)((k - 5) * (k - 5)) / (2.0 * 1.5 * 1.5)); sum += g[k]; }
-        for (int k = 0; k < 11; k++) prm.g[k] = g[k] / sum;
-    }
-    const GhLossParts np = GhLossParts::of(width, height);
-    double* sums = reinterpret_cast<double*>(workspace);
-    double* part_presum = sums + GH_LS_COUNT;
-    double* part_pointwise = part_presum + np.rb;
-    double* part_main = part_pointwise + 3 * (size_t)np.pb;
-    float* dmaps = reinterpret_cast<float*>(part_main + np.mb);
-    const size_t plane = (size_t)width * height;
-    const cudaError_t e = cudaMemsetAsync(sums, 0, GH_LS_COUNT * sizeof(double), stream);     // sums + tickets
-    if (e != cudaSuccess) return gh_cuda_status("gh_image_loss", "memset(partial sums)", e);
-    const int rb = np.rb, pb = np.pb;
-    const dim3 grid((width + GH_LT - 1) / GH_LT, (height + GH_LT - 1) / GH_LT), block(256);
-    if (deterministic) {
-        gh_loss_presum_kernel<true><<<rb, 256, 0, stream>>>(gt_orient_conf, plane, sums, part_presum);
-        gh_loss_pointwise_kernel<true><<<pb, 256, 0, stream>>>(prm, out_color, gt_image, gt_mask, gt_orient_angle, gt_orient_conf,
-                                                               sums, dL_dout, part_pointwise);
-        gh_loss_main_kernel<4, true><<<grid, block, 0, stream>>>(prm, out_color, gt_image, gt_mask, sums, dmaps, part_main);
-    } else {
-        gh_loss_presum_kernel<false><<<rb, 256, 0, stream>>>(gt_orient_conf, plane, sums, nullptr);
-        gh_loss_pointwise_kernel<false><<<pb, 256, 0, stream>>>(prm, out_color, gt_image, gt_mask, gt_orient_angle, gt_orient_conf,
-                                                                sums, dL_dout, nullptr);
-        // 4 CTAs per SM (64 registers)
-        gh_loss_main_kernel<4, false><<<grid, block, 0, stream>>>(prm, out_color, gt_image, gt_mask, sums, dmaps, nullptr);
-    }
-    gh_loss_ssim_bwd_kernel<4><<<grid, block, 0, stream>>>(prm, out_color, gt_image, gt_mask, dmaps, dL_dout);
-    gh_loss_finalize_kernel<<<rb, 256, 0, stream>>>(prm, sums, losses, dL_dout);
-    return gh_launch_status("gh_image_loss", 5);
+    return gh_image_loss_run("gh_image_loss", width, height, GH_LOSS_STAGE_APPEARANCE, 0u, out_color, gt_image, gt_mask,
+                             gt_orient_angle, gt_orient_conf, lambda_dl1, lambda_dssim, lambda_dmask, lambda_dorient,
+                             workspace, losses, dL_dout, stream_, deterministic);
+}
+
+extern "C" int gh_image_loss_stage(int width, int height, int stage, unsigned options, const float* out_color,
+                                   const float* gt_image, const float* gt_mask, const float* gt_orient_angle,
+                                   const float* gt_orient_conf, float lambda_dl1, float lambda_dssim,
+                                   float lambda_dmask, float lambda_dorient, void* workspace, float* losses,
+                                   float* dL_dout, gh_stream_t stream_, int deterministic)
+{
+    gh_clear_error();
+    const unsigned known = GH_LOSS_ORIENT_UNIT_WEIGHT | GH_LOSS_ORIENT_NO_CONF;
+    if (stage < GH_LOSS_STAGE_APPEARANCE || stage > GH_LOSS_STAGE_LATENT_STRANDS)
+        return gh_set_error(GH_E_INVALID_ARG, "gh_image_loss_stage: unknown stage %d", stage);
+    if (options & ~known)
+        return gh_set_error(GH_E_INVALID_ARG, "gh_image_loss_stage: unknown option bits 0x%x", options & ~known);
+    if (stage == GH_LOSS_STAGE_APPEARANCE && options)
+        return gh_set_error(GH_E_INVALID_ARG, "gh_image_loss_stage: the appearance stage takes no options");
+    if (stage == GH_LOSS_STAGE_LATENT_STRANDS && lambda_dssim != 0.f)
+        return gh_set_error(GH_E_INVALID_ARG, "gh_image_loss_stage: the latent-strand stage has no SSIM term "
+                                              "(lambda_dssim must be 0)");
+    return gh_image_loss_run("gh_image_loss_stage", width, height, stage, options, out_color, gt_image, gt_mask,
+                             gt_orient_angle, gt_orient_conf, lambda_dl1, lambda_dssim, lambda_dmask, lambda_dorient,
+                             workspace, losses, dL_dout, stream_, deterministic);
 }

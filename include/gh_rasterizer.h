@@ -240,6 +240,42 @@ int gh_image_loss(int width, int height, const float* out_color, const float* gt
                   void* workspace, float* losses, float* dL_dout, gh_stream_t stream, int deterministic);
 
 /*
+ * The image loss of each training stage, in the same kernels as gh_image_loss (inputs, workspace and losses[8] as
+ * there; gh_image_loss_workspace_size serves every stage):
+ *   GH_LOSS_STAGE_APPEARANCE      src/train_gaussians.py:126-140, bit-identical to gh_image_loss
+ *   GH_LOSS_STAGE_STRANDS         src/train_strands.py:128-147: Ll1 = l1_loss(image, gt_image) and
+ *                                 Lssim = 1 - ssim(image, gt_image), both unmasked; Lmask and Lorient as appearance
+ *   GH_LOSS_STAGE_LATENT_STRANDS  src/train_latent_strands.py:130-152: Ll1 unmasked, no SSIM term,
+ *                                 LCE = l1_loss(mask[:1], gt_mask[:1]) (channel 3 only), LOR as Lorient
+ * options (strand stages only):
+ *   GH_LOSS_ORIENT_UNIT_WEIGHT    opt.use_gt_orient_conf == False: orientation weight 1, sum of weights W H;
+ *                                 gt_orient_conf may then be NULL and is not read
+ *   GH_LOSS_ORIENT_NO_CONF        opt.train_orient_conf == False: or_loss(..., confs=None), no conf factor and no
+ *                                 log term; channel 8 of dL_dout is exactly 0
+ * losses[8]: total, Ll1, Lssim, Lmask, Lorient, sum of orientation weights, Lorient-was-NaN, slot 7.  Stage 2: slot 2
+ *   is 0, slot 3 holds LCE, slot 7 the terms replaced by 0 because they were NaN as a float bitmask (1 Ll1, 2 LCE);
+ *   slot 7 is 0 in the other stages.  total is the reference's sum without its prior term (lambda_dsds Lsds or
+ *   lambda_dsds LDF), in the reference's order, so a trainer that adds that term afterwards gets the reference's total.
+ * dL_dout: every element written.  Channels 7 and 9 are 0; in stage 2 channel 4 is 0; a replaced term contributes
+ *   exactly 0: Lorient / LOR channels 5, 6, 8, and in stage 2 Ll1 channels 0..2 and LCE channel 3.  Stage 1 replaces
+ *   only Lorient, like the reference: a NaN Ll1 or Lssim stays NaN in the total.
+ * deterministic: as gh_image_loss.
+ * Refused with GH_E_INVALID_ARG before any CUDA call: a stage outside 0..2, option bits with stage 0, unknown option
+ *   bits, lambda_dssim != 0 with stage 2, a NULL gt_orient_conf without GH_LOSS_ORIENT_UNIT_WEIGHT, and everything
+ *   gh_image_loss refuses.
+ */
+#define GH_LOSS_STAGE_APPEARANCE     0
+#define GH_LOSS_STAGE_STRANDS        1
+#define GH_LOSS_STAGE_LATENT_STRANDS 2
+#define GH_LOSS_ORIENT_UNIT_WEIGHT   1u
+#define GH_LOSS_ORIENT_NO_CONF       2u
+int gh_image_loss_stage(int width, int height, int stage, unsigned options,
+                        const float* out_color, const float* gt_image, const float* gt_mask,
+                        const float* gt_orient_angle, const float* gt_orient_conf,
+                        float lambda_dl1, float lambda_dssim, float lambda_dmask, float lambda_dorient,
+                        void* workspace, float* losses, float* dL_dout, gh_stream_t stream, int deterministic);
+
+/*
  * Multi-GPU (SURVEY.md 8e): sum a float32 buffer that lives in SYMMETRIC memory (the same allocation on
  * every GPU of the node, each mapped into every process, e.g. torch.distributed._symmetric_memory) over
  * all ranks, in place, with one kernel per rank that reads and writes its peers' copies through NVLink.

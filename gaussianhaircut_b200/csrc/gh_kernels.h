@@ -104,6 +104,9 @@ int gh_forward_phase1_capturable(const char* who, int P, int width, int height, 
                                         status, num_rendered_out, stream,
                                         [](const void* f, const GhGeomWS& g, const GhImgWS& i, int gx, int gy) { (*static_cast<const F*>(f))(g, i, gx, gy); }, &bin);
 }
+// the strand geometry kernels of gh_strands.cu (gh_strand_midpoints, gh_strand_backward) without their argument checks
+void gh_launch_strand_midpoints(int S, int L, const float* origins, const float* dirs, float* xyz, cudaStream_t stream);
+void gh_launch_strand_backward(int S, int L, const float* d_xyz, float* d_dirs, unsigned int* nan_flag, cudaStream_t stream);
 // shared refusals of every capturable entry point (before any launch): debug != 0 and calls while the stage timer is on
 // (both synchronise with the host)
 int gh_check_capturable(const char* who, int debug);

@@ -141,6 +141,19 @@ gh_project_forward_tan_kernel(GhProjArgs A, const float* __restrict__ tan_fov, f
                                          tile_count, gx, gy);
 }
 
+// The strand rows of gh_hair_strands_forward_binned_capturable: gh_project_forward_tan_kernel for polyline segments.
+// The caller offsets every output and workspace pointer by the head block's rows.
+__global__ void __launch_bounds__(GH_PJ_THREADS)
+gh_project_forward_strand_tan_kernel(GhProjArgs A, const float* __restrict__ tan_fov, float* __restrict__ means2D,
+                                     float* __restrict__ colors, float* __restrict__ opac_out, float* __restrict__ conic_out,
+                                     unsigned char* __restrict__ mask_out, int* __restrict__ radii, GhGeo* __restrict__ geo,
+                                     float* __restrict__ depth, uint32_t* __restrict__ tile_count, int gx, int gy)
+{
+    A.tanx = __ldg(tan_fov); A.tany = __ldg(tan_fov + 1);
+    gh_project_forward_body<true, true>(A, means2D, colors, opac_out, conic_out, nullptr, mask_out, radii, geo, depth,
+                                        tile_count, gx, gy);
+}
+
 // ------------------------------------------------------------------------------------------------ backward
 // Incoming gradients: either the four API-shaped tensors of gh_backward (dL_dmean2D (P,3) NDC units,
 // dL_dconic (P,4) = (d/da, HALF d/db, unused, d/dc), dL_dcolor (P,10), dL_dopacity (P)), or -- when acc16 is
@@ -366,6 +379,19 @@ GhProjArgs gh_proj_args(int P, int width, int height, const float* xyz, const fl
 // flag bit 10: the strand instantiation (Gaussian i = segment i of a polyline, geometry derived from dirs[i])
 bool gh_proj_strand(unsigned int flags) { return (flags >> 10) & 1u; }
 
+// the row counts of the gh_hair_strands_*_capturable entry points: n_head head rows, then S * L segment rows
+int gh_strand_rows_check(const char* who, int n_head, int S, int L, bool need_strands)
+{
+    if (n_head < 0) return gh_set_error(GH_E_INVALID_ARG, "%s: n_head must not be negative", who);
+    if (S < 0 || L < 0 || (need_strands && (S == 0 || L == 0)))
+        return gh_set_error(GH_E_INVALID_ARG, "%s: S and L must be %s", who, need_strands ? "positive" : "non-negative");
+    const unsigned long long seg = (unsigned long long)S * (unsigned long long)L;
+    if (3ull * seg > 0x7fffffffull) return gh_set_error(GH_E_INVALID_ARG, "%s: S * L overflows int (3 * S * L must stay below 2^31)", who);
+    if ((unsigned long long)n_head + seg > 0x7fffffffull) return gh_set_error(GH_E_INVALID_ARG, "%s: n_head + S * L overflows int", who);
+    if (n_head == 0 && seg == 0) return gh_set_error(GH_E_INVALID_ARG, "%s: nothing to render (n_head == 0 and S * L == 0)", who);
+    return GH_OK;
+}
+
 }  // namespace
 
 extern "C" int gh_project_workspace_size(int P, size_t* bytes)
@@ -576,4 +602,108 @@ extern "C" int gh_project_backward_capturable(
         d_xyz, d_scaling, d_rotation, d_dirs, d_features_dc, d_features_rest, d_opacity, d_label, d_orient_conf,
         d_means2D, partial, ticket, d_camera, nan_flag);
     return gh_launch_status(who, 1);
+}
+
+// ------------------------------------------------------------------------------------------------ capturable, strands
+// The strand model behind its frozen head block (render_hair_strands) in one capturable first phase over P = n_head +
+// S * L rows -- head rows first, then the segments, the row order of the eager path -- and the records-mode parameter
+// backward of the segment rows.  The head block is frozen and the cameras are not trained: no head-row or camera
+// gradients.
+extern "C" int gh_hair_strands_forward_binned_capturable(
+    int n_head, int S, int L, int width, int height,
+    const float* head_xyz, const float* head_scaling, const float* head_rotation,
+    const float* head_features_dc, const float* head_features_rest, const float* head_opacity,
+    unsigned int head_flags, float head_det_eps,
+    const float* origins, const float* dirs, const float* scale,
+    const float* features_dc, const float* features_rest, const float* orient_conf,
+    unsigned int flags, float det_eps,
+    const float* viewmatrix, const float* projmatrix, const float* campos,
+    const float* tan_fov, float scale_modifier, int sh_degree,
+    float* midpoints,
+    float* means2D, float* colors, float* opacities, float* conic, unsigned char* visible,
+    int* radii, char* geom_buffer, char* img_buffer, char* binning_buffer, long long capacity,
+    unsigned int* status, unsigned int* num_rendered, int debug, gh_stream_t stream_)
+{
+    const char* who = "gh_hair_strands_forward_binned_capturable";
+    cudaStream_t stream = (cudaStream_t)stream_;
+    gh_clear_error();
+    int rc = gh_check_capturable(who, debug);
+    if (rc == GH_OK) rc = gh_check_capacity(who, capacity);
+    if (rc == GH_OK) rc = gh_strand_rows_check(who, n_head, S, L, false);
+    if (rc != GH_OK) return rc;
+    if (!tan_fov) return gh_set_error(GH_E_INVALID_ARG, "%s: tan_fov (device float[2]) is required", who);
+    if (!status) return gh_set_error(GH_E_INVALID_ARG, "%s: status (device uint32) is required", who);
+    if (gh_proj_strand(head_flags)) return gh_set_error(GH_E_INVALID_ARG, "%s: head_flags must not set the strand bit", who);
+    if (!gh_proj_strand(flags)) return gh_set_error(GH_E_INVALID_ARG, "%s: flags must set the strand bit (10)", who);
+    const int n_seg = S * L, P = n_head + n_seg;
+    // (the kernels read tan(fov / 2) from tan_fov; 1 stands in for it in the host-side checks)
+    GhProjArgs Ah = gh_proj_args(n_head, width, height, head_xyz, head_scaling, head_rotation, nullptr, head_features_dc,
+                                 head_features_rest, head_opacity, nullptr, nullptr, viewmatrix, projmatrix, campos,
+                                 1.f, 1.f, scale_modifier, sh_degree, head_flags, head_det_eps);
+    GhProjArgs As = gh_proj_args(n_seg, width, height, midpoints, scale, nullptr, dirs, features_dc, features_rest, nullptr,
+                                 nullptr, orient_conf, viewmatrix, projmatrix, campos, 1.f, 1.f, scale_modifier, sh_degree,
+                                 flags, det_eps);
+    if (n_head > 0 && (rc = gh_proj_check(Ah, who, false)) != GH_OK) return rc;
+    if (n_seg > 0) {
+        if (!origins || !midpoints) return gh_set_error(GH_E_INVALID_ARG, "%s: origins and midpoints are required", who);
+        if ((rc = gh_proj_check(As, who, true)) != GH_OK) return rc;
+    }
+    if (!means2D || !colors || !opacities || !conic || !visible || !radii || !geom_buffer || !img_buffer || !binning_buffer)
+        return gh_set_error(GH_E_INVALID_ARG, "%s: missing output pointer", who);
+    if ((size_t)colors & 7) return gh_set_error(GH_E_INVALID_ARG, "%s: colors must be 8-byte aligned", who);
+    return gh_forward_phase1_capturable(who, P, width, height, radii, geom_buffer, img_buffer, binning_buffer, capacity,
+                                        status, num_rendered, stream, [&](const GhGeomWS& geom, const GhImgWS& img, int gx, int gy) {
+        if (n_head > 0) {
+            gh_project_forward_tan_kernel<<<(n_head + GH_PJ_THREADS - 1) / GH_PJ_THREADS, GH_PJ_THREADS, 0, stream>>>(
+                Ah, tan_fov, means2D, colors, opacities, conic, visible, radii, geom.geo, geom.depth, img.tile_count, gx, gy);
+            gh_count_launches(1);
+        }
+        if (n_seg > 0) {
+            // the midpoints in segment order (bit-identical to the eager path's), then the segment rows behind the head's
+            gh_launch_strand_midpoints(S, L, origins, dirs, midpoints, stream);
+            const size_t h = (size_t)n_head;
+            gh_project_forward_strand_tan_kernel<<<(n_seg + GH_PJ_THREADS - 1) / GH_PJ_THREADS, GH_PJ_THREADS, 0, stream>>>(
+                As, tan_fov, means2D + 3 * h, colors + GH_NUM_CHANNELS * h, opacities + h, conic + 3 * h, visible + h,
+                radii + h, geom.geo + h, geom.depth + h, img.tile_count, gx, gy);
+            gh_count_launches(2);
+        }
+    });
+}
+
+extern "C" int gh_hair_strands_backward_capturable(
+    int n_head, int S, int L, int width, int height,
+    const float* midpoints, const float* dirs, const float* scale,
+    const float* features_dc, const float* features_rest, const float* orient_conf,
+    unsigned int flags, float det_eps,
+    const float* viewmatrix, const float* projmatrix, const float* campos,
+    const float* tan_fov, float scale_modifier, int sh_degree,
+    const unsigned char* visible, const char* geom_buffer,
+    float* d_xyz, float* d_dirs, float* d_features_dc, float* d_features_rest, float* d_orient_conf,
+    unsigned int* nan_flag, int debug, gh_stream_t stream_)
+{
+    const char* who = "gh_hair_strands_backward_capturable";
+    cudaStream_t stream = (cudaStream_t)stream_;
+    gh_clear_error();
+    int rc = gh_check_capturable(who, debug);
+    if (rc == GH_OK) rc = gh_strand_rows_check(who, n_head, S, L, true);
+    if (rc != GH_OK) return rc;
+    if (!tan_fov) return gh_set_error(GH_E_INVALID_ARG, "%s: tan_fov (device float[2]) is required", who);
+    if (!gh_proj_strand(flags)) return gh_set_error(GH_E_INVALID_ARG, "%s: flags must set the strand bit (10)", who);
+    const int n_seg = S * L;
+    GhProjArgs A = gh_proj_args(n_seg, width, height, midpoints, scale, nullptr, dirs, features_dc, features_rest, nullptr,
+                                nullptr, orient_conf, viewmatrix, projmatrix, campos, 1.f, 1.f, scale_modifier, sh_degree,
+                                flags, det_eps);
+    rc = gh_proj_check(A, who, true);
+    if (rc != GH_OK) return rc;
+    if (!visible || !geom_buffer || !d_xyz || !d_dirs || !d_features_dc || !d_features_rest)
+        return gh_set_error(GH_E_INVALID_ARG, "%s: missing mandatory pointer", who);
+    // the blend backward's accumulation records of the segment rows, in the geometry workspace of all P rows
+    const size_t h = (size_t)n_head;
+    const float* acc16 = GhGeomWS::carve(const_cast<char*>(geom_buffer), h + (size_t)n_seg).acc16 + 16 * h;
+    gh_project_backward_tan_kernel<true><<<(n_seg + GH_PJ_THREADS - 1) / GH_PJ_THREADS, GH_PJ_THREADS, 0, stream>>>(
+        A, tan_fov, visible + h, acc16, nullptr, nullptr, nullptr, nullptr,
+        d_xyz, nullptr, nullptr, d_dirs, d_features_dc, d_features_rest, nullptr, nullptr, d_orient_conf,
+        nullptr, nullptr, nullptr, nullptr, nan_flag);
+    gh_launch_strand_backward(S, L, d_xyz, d_dirs, nan_flag, stream);
+    return gh_launch_status(who, 2);
 }

@@ -92,6 +92,17 @@ int gh_strand_check(int S, int L, const char* who)
 
 }  // namespace
 
+// the two kernels for entry points outside this file (gh_hair_strands_*_capturable); S, L checked by the caller
+void gh_launch_strand_midpoints(int S, int L, const float* origins, const float* dirs, float* xyz, cudaStream_t stream)
+{
+    gh_strand_midpoints_kernel<<<(3 * S + GH_ST_THREADS - 1) / GH_ST_THREADS, GH_ST_THREADS, 0, stream>>>(S, L, origins, dirs, xyz);
+}
+
+void gh_launch_strand_backward(int S, int L, const float* d_xyz, float* d_dirs, unsigned int* nan_flag, cudaStream_t stream)
+{
+    gh_strand_backward_kernel<<<(S + GH_ST_WARPS - 1) / GH_ST_WARPS, GH_ST_THREADS, 0, stream>>>(S, L, d_xyz, d_dirs, nan_flag);
+}
+
 extern "C" int gh_strand_midpoints(int S, int L, const float* origins, const float* dirs, float* xyz, gh_stream_t stream_)
 {
     cudaStream_t stream = (cudaStream_t)stream_;

@@ -162,7 +162,9 @@ def strand_image_loss(render: torch.Tensor, gt_image: torch.Tensor, gt_mask: tor
     `use_gt_orient_conf` / `train_orient_conf` are the trainer's `opt` fields; with use_gt_orient_conf=False
     gt_orient_conf may be None.  Returns (loss, parts): `loss` is differentiable w.r.t. `render`; `parts` holds Ll1,
     Lssim, Lmask, Lorient and orient_nan as 0-dim device tensors (no host sync).  A NaN Ll1 or Lssim stays NaN in
-    the loss, as in the reference.  Add `Lsds * opt.lambda_dsds` to the loss for the reference's total."""
+    the loss, as in the reference.  Add `Lsds * opt.lambda_dsds` to the loss for the reference's total.
+    graphs.CapturedStrandStep runs this loss inside the captured train_strands.py iteration; there the trainer passes
+    the prior term's `_dirs` gradient to step(dirs_grad=...) instead."""
     total, p = HairImageLoss.apply(render, gt_image, gt_mask, gt_orient_angle, gt_orient_conf,
                                    lambda_dl1, lambda_dssim, lambda_dmask, lambda_dorient, "strands",
                                    use_gt_orient_conf, train_orient_conf)

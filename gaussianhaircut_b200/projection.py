@@ -312,3 +312,99 @@ def strand_backward(S: int, L: int, d_xyz: torch.Tensor, d_dirs: torch.Tensor, n
     with torch.cuda.device(dev):
         _capi.check(lib.gh_strand_backward(S, L, _ptr(d_xyz), _ptr(d_dirs), _ptr(nan_flag), _stream(dev)))
     return d_dirs.view(S, L, 3)
+
+
+# ------------------------------------------------------------------------------------------------- capturable strands
+class StrandInputs:
+    """The (detached, contiguous) tensors of one capturable strand render (head block + strand model), kept between the
+    forward and the backward."""
+    __slots__ = ("n_head", "S", "L", "W", "H", "head", "origins", "dirs", "scale", "f_dc", "f_rest", "conf", "V", "Pm",
+                 "campos", "tan_fov", "mod", "sh_degree", "device")
+
+    @property
+    def P(self) -> int:
+        return self.n_head + self.S * self.L
+
+    def common(self):
+        """The arguments shared by the two gh_hair_strands_*_capturable entry points after the row counts."""
+        return (_ptr(self.dirs), _ptr(self.scale), _ptr(self.f_dc), _ptr(self.f_rest), _ptr(self.conf),
+                encode_flags(HAIR_STRANDS), float(HAIR_STRANDS["det_eps"]), _ptr(self.V), _ptr(self.Pm), _ptr(self.campos),
+                _ptr(self.tan_fov), self.mod, self.sh_degree)
+
+
+def pack_strand_inputs(head, origins, dirs, scale, f_dc, f_rest, conf, viewmatrix, projmatrix, campos, tan_fov,
+                       width: int, height: int, sh_degree: int, scaling_modifier: float) -> StrandInputs:
+    """`head`: the frozen head block (renderer._head_block: xyz, scaling, rotation, opacity, f_dc, f_rest) or None;
+    `dirs` (S,L,3) segment vectors, `origins` (S,1,3), `scale` the (1,) strand thickness, f_dc / f_rest / conf with
+    S*L rows; the camera tensors and the (2,) `tan_fov` on the device."""
+    dev = dirs.device
+    if dirs.ndim != 3 or dirs.shape[-1] != 3:
+        raise RuntimeError(f"projection: dirs must be (S, L, 3), got {tuple(dirs.shape)}")
+    sp = StrandInputs()
+    sp.device = dev
+    sp.S, sp.L, sp.W, sp.H = int(dirs.shape[0]), int(dirs.shape[1]), int(width), int(height)
+    sp.head = None
+    if head is not None and int(head["xyz"].shape[0]) > 0:
+        sp.head = {k: _f32(head[k], "head " + k, dev, align=16 if k == "rotation" else 4)
+                   for k in ("xyz", "scaling", "rotation", "f_dc", "f_rest", "opacity")}
+    sp.n_head = 0 if sp.head is None else int(sp.head["xyz"].shape[0])
+    sp.origins, sp.dirs = _f32(origins, "pts_origins", dev), _f32(dirs, "dirs", dev)
+    sp.scale = _f32(scale, "scale", dev)
+    sp.f_dc, sp.f_rest, sp.conf = _f32(f_dc, "features_dc", dev), _f32(f_rest, "features_rest", dev), _f32(conf, "orient_conf", dev)
+    sp.V, sp.Pm, sp.campos = _f32(viewmatrix, "viewmatrix", dev), _f32(projmatrix, "projmatrix", dev), _f32(campos, "campos", dev)
+    sp.tan_fov = _f32(tan_fov, "tan_fov", dev)
+    sp.mod, sp.sh_degree = float(scaling_modifier), int(sh_degree)
+    n = sp.S * sp.L
+    if sp.origins is None or sp.origins.numel() != 3 * sp.S:
+        raise RuntimeError(f"projection: pts_origins must be (S, 1, 3) = ({sp.S}, 1, 3)")
+    if sp.scale is None or sp.scale.numel() != 1:
+        raise RuntimeError("projection: the strand thickness must be a (1,) tensor")
+    for name, t, per in (("features_dc", sp.f_dc, 3), ("orient_conf", sp.conf, 1)):
+        if t is None or t.numel() != n * per:
+            raise RuntimeError(f"projection: '{name}' must have {per} floats per segment (S*L = {n} rows)")
+    if sp.sh_degree > 0 and (sp.f_rest is None or sp.f_rest.numel() != n * 45):
+        raise RuntimeError("projection: 'features_rest' must be (S*L, 15, 3) for sh_degree > 0")
+    return sp
+
+
+def hair_strands_forward_binned_capturable(sp: StrandInputs, binning: torch.Tensor, capacity: int, status: torch.Tensor,
+                                           num_rendered: Optional[torch.Tensor] = None):
+    """gh_hair_strands_forward_binned_capturable: the capturable first phase of render_hair_strands over P = n_head +
+    S*L rows (head rows first).  -> (out dict as project_forward with P rows, radii, geomBuffer, imgBuffer, midpoints
+    (S*L,3)); continue with `_C.forward_render_capturable`.  No host synchronisation."""
+    from . import _C
+    lib = _capi.load()
+    dev, P = sp.device, sp.P
+    out = alloc_outputs(P, dev)
+    geom, img, radii = _C.alloc_forward_workspaces(P, sp.W, sp.H, dev)
+    mid = empty_rows(sp.S * sp.L, (3,), torch.float32, dev)
+    hd = sp.head or {}
+    h = lambda k: _ptr(hd.get(k))  # noqa: E731
+    with torch.cuda.device(dev):
+        _capi.check(lib.gh_hair_strands_forward_binned_capturable(
+            sp.n_head, sp.S, sp.L, sp.W, sp.H, h("xyz"), h("scaling"), h("rotation"), h("f_dc"), h("f_rest"), h("opacity"),
+            encode_flags(HEAD_PRECOMP), float(HEAD_PRECOMP["det_eps"]), _ptr(sp.origins), *sp.common(), _ptr(mid),
+            _ptr(out["means2D"]), _ptr(out["colors"]), _ptr(out["opacity"]), _ptr(out["conic"]), _ptr(out["visible"]),
+            _ptr(radii), _ptr(geom), _ptr(img), _ptr(binning), int(capacity), _ptr(status), _ptr(num_rendered), 0,
+            _stream(dev)))
+    return out, radii, geom, img, mid
+
+
+def hair_strands_backward_capturable(sp: StrandInputs, midpoints: torch.Tensor, visible: torch.Tensor,
+                                     geom_buffer: torch.Tensor, nan_flag: Optional[torch.Tensor] = None):
+    """gh_hair_strands_backward_capturable, after `_C.backward_records_capturable` over all P rows: the gradients of the
+    strand model's parameters from the accumulation records of its rows -> dict(dirs (S,L,3), f_dc (S*L,1,3), f_rest
+    (S*L,15,3), conf (S*L,1)).  `nan_flag` as in project_backward."""
+    _check_no_strand_arena()
+    lib = _capi.load()
+    dev, n = sp.device, sp.S * sp.L
+    g = {k: empty_rows(n, shape, torch.float32, dev) for k, shape in (("xyz", (3,)), ("dirs", (3,)), ("f_dc", (1, 3)),
+                                                                      ("f_rest", (15, 3)), ("conf", (1,)))}
+    with torch.cuda.device(dev):
+        _capi.check(lib.gh_hair_strands_backward_capturable(
+            sp.n_head, sp.S, sp.L, sp.W, sp.H, _ptr(midpoints), *sp.common(), _ptr(visible), _ptr(geom_buffer),
+            _ptr(g["xyz"]), _ptr(g["dirs"]), _ptr(g["f_dc"]), _ptr(g["f_rest"]), _ptr(g["conf"]), _ptr(nan_flag), 0,
+            _stream(dev)))
+    g["dirs"] = g["dirs"].view(sp.S, sp.L, 3)
+    del g["xyz"]
+    return g

@@ -26,7 +26,8 @@ import torch.nn.functional as F
 from . import _C, projection
 from ._alloc import empty_rows
 
-__all__ = ["render", "render_hair", "render_hair_strands", "render_raw", "render_raw_capturable", "set_nan_flag"]
+__all__ = ["render", "render_hair", "render_hair_strands", "render_hair_strands_capturable", "render_raw",
+           "render_raw_capturable", "set_nan_flag"]
 
 _EMPTY = torch.Tensor([])
 
@@ -232,6 +233,65 @@ def render_raw_capturable(camera: Dict[str, torch.Tensor], pc, bg_color: torch.T
     return renders, radii, viewspace
 
 
+class _CapturableStrandRender(torch.autograd.Function):
+    """The capturable twin of _FusedRender for render_hair_strands: (dirs, f_dc, f_rest, conf, static) -> (raw image,
+    radii) over the head block and the strand rows, with the gradients of the four strand parameters.  `static` holds
+    the packed inputs (projection.StrandInputs), the binning buffer, its capacity, the status word and num_rendered."""
+
+    @staticmethod
+    def forward(ctx, dirs, f_dc, f_rest, conf, static):
+        st = static
+        sp = projection.pack_strand_inputs(st["head"], st["origins"], dirs, st["scale"], f_dc, f_rest, conf,
+                                           *st["camera"], st["W"], st["H"], st["sh_degree"], st["mod"])
+        out, radii, geom, img, mid = projection.hair_strands_forward_binned_capturable(
+            sp, st["binning"], st["capacity"], st["status"], st["num_rendered"])
+        color = _C.forward_render_capturable(st["bg"], out["colors"], geom, st["binning"], img, st["capacity"], sp.H, sp.W)
+        ctx.sp, ctx.st = sp, st
+        ctx.bufs = (out["colors"], out["visible"], radii, geom, img, mid)
+        ctx.mark_non_differentiable(radii)
+        return color, radii
+
+    @staticmethod
+    def backward(ctx, g_color, _g_radii):
+        st = ctx.st
+        colors, visible, radii, geom, img, mid = ctx.bufs
+        _C.backward_records_capturable(st["bg"], colors, radii, geom, st["binning"], img, st["capacity"], g_color)
+        g = projection.hair_strands_backward_capturable(ctx.sp, mid, visible, geom, nan_flag=_NAN_FLAG["t"])
+        need = ctx.needs_input_grad
+        return (g["dirs"] if need[0] else None, g["f_dc"] if need[1] else None, g["f_rest"] if need[2] else None,
+                g["conf"] if need[3] else None, None)
+
+
+def render_hair_strands_capturable(camera: Dict[str, torch.Tensor], pc, pc_hair, bg_color: torch.Tensor, width: int,
+                                   height: int, binning: torch.Tensor, capacity: int, status: torch.Tensor,
+                                   num_rendered: Optional[torch.Tensor] = None, scaling_modifier: float = 1.0):
+    """`render_hair_strands` for CUDA-graph capture (graphs.CapturedStrandStep): the frozen head block of `pc` (None or
+    an empty block: hair only) followed by the segments of the strand model `pc_hair`, with no host synchronisation.
+    `camera`, `binning`, `capacity`, `status` and `num_rendered` as in render_raw_capturable (no camera tensor may
+    require grad: the strand stage does not train its cameras).  -> (raw (10,H,W) image, radii (n_head + S*L,)).
+    Gradients land in `.grad` of `_dirs`, `_features_dc`, `_features_rest` and `_orient_conf`; set_nan_flag() works as
+    with render_hair_strands.  With the same inputs, image, radii and (deterministic mode) gradients are bit-identical
+    to render_hair_strands'."""
+    for k in ("viewmatrix", "projmatrix", "campos", "tan_fov"):
+        if camera[k].requires_grad:
+            raise RuntimeError(f"render_hair_strands_capturable: camera tensor '{k}' requires grad; trainable cameras are "
+                               "not supported")
+    projection._check_no_strand_arena()
+    dirs = pc_hair._dirs
+    if dirs.ndim != 3 or dirs.shape[-1] != 3 or dirs.shape[0] < 1 or dirs.shape[1] < 1:
+        raise RuntimeError(f"render_hair_strands_capturable: _dirs must be (S, L, 3) with S, L >= 1, got {tuple(dirs.shape)}")
+    scale = pc_hair.scale
+    if not isinstance(scale, torch.Tensor):
+        raise RuntimeError("render_hair_strands_capturable: pc_hair.scale must be a (1,) device tensor (a captured "
+                           "launch keeps its address)")
+    head = _head_block(pc) if pc is not None else None
+    st = {"W": int(width), "H": int(height), "bg": bg_color, "mod": float(scaling_modifier),
+          "sh_degree": int(pc_hair.active_sh_degree), "head": head, "origins": pc_hair.pts_origins, "scale": scale.detach(),
+          "camera": (camera["viewmatrix"], camera["projmatrix"], camera["campos"], camera["tan_fov"]),
+          "binning": binning, "capacity": int(capacity), "status": status, "num_rendered": num_rendered}
+    return _CapturableStrandRender.apply(dirs, pc_hair._features_dc, pc_hair._features_rest, pc_hair._orient_conf, st)
+
+
 def _post(renders: torch.Tensor, radii: torch.Tensor, viewspace: torch.Tensor) -> Dict[str, torch.Tensor]:
     """The reference's epilogue (gaussian_renderer/__init__.py:98-113)."""
     rendered_image, rendered_mask, rendered_cov2D, rendered_orient_conf, _ = renders.split([3, 2, 3, 1, 1], dim=0)
@@ -333,7 +393,11 @@ def render_hair_strands(viewpoint_camera, pc, pc_hair, pipe, bg_color: torch.Ten
 
     This does NOT refresh `pc_hair._pts`, `_xyz` or `_rotation`: a trainer that calls `capture()` (which saves them)
     runs the model's own initialize_gaussians_hair() under torch.no_grad() first.  The strand model has no
-    gradient-arena layout: an installed arena (projection.set_gradient_arena) raises."""
+    gradient-arena layout: an installed arena (projection.set_gradient_arena) raises.
+
+    render_hair_strands_capturable is the CUDA-graph form (graphs.CapturedStrandStep captures the whole train_strands.py
+    iteration with it): one first phase over the head and strand rows, a records-mode backward, and the same image,
+    radii and deterministic-mode gradients as this function."""
     projection._check_no_strand_arena()
     dirs = pc_hair._dirs
     if dirs.ndim != 3 or dirs.shape[-1] != 3 or dirs.shape[1] < 1:

@@ -449,6 +449,54 @@ int gh_adam_step_capturable(int n_groups, float* const* params, const float* con
                             unsigned int* nan_flag, const unsigned int* skip_flag, int debug, gh_stream_t stream);
 
 /*
+ * Capturable strand iteration (DESIGN §19): render_hair_strands -- the frozen head block of n_head Gaussians followed by
+ * the S * L segments of a strand model (strand-major) -- under the contract of the capturable block above (tan fov
+ * from the device float[2] `tan_fov`, R only on the device, a binning buffer of `capacity` records, the overflow
+ * contract of GH_STATUS_BINNING_OVERFLOW; debug != 0 and the stage timer are refused before any launch).  The
+ * P = n_head + S * L rows keep the order of the eager path (head rows first), so that with the same inputs radii, keys,
+ * the sorted lists and the image are bit-identical to it.  Continue with gh_forward_render_capturable and
+ * gh_backward_capturable over all P rows (colors, geom/img/binning buffers of this call).
+ *
+ * gh_hair_strands_forward_binned_capturable: gh_strand_midpoints into `midpoints` (S*L,3) (the strand rows' means),
+ *   the head rows projected with `head_flags` (no strand bit; the head block has no dirs, label or orient_conf) and
+ *   `head_det_eps`, the segment rows with `flags` (strand bit set; `scale` = one device float, the strand thickness)
+ *   and `det_eps`, then one tile histogram, scan, capacity guard and emit over all P rows.  Outputs as in
+ *   gh_project_forward_binned_capturable, with P rows.  n_head >= 0, S, L >= 0, 3 * S * L and n_head + S * L below 2^31,
+ *   P > 0; with S * L == 0 only the head block is rendered.  `status` is required, num_rendered (device uint32) may be
+ *   NULL.
+ * gh_hair_strands_backward_capturable: the parameter backward of the segment rows alone, after gh_backward_capturable:
+ *   the strand-mode projection backward reads the accumulation records of rows [n_head, P) in place from
+ *   `geom_buffer` (the geometry workspace of the P-row forward; `visible` has P rows), writes dL/d midpoint to d_xyz
+ *   (S*L,3, scratch) and the gradients of d_dirs, d_features_dc, d_features_rest, d_orient_conf (may be NULL), then
+ *   gh_strand_backward completes d_dirs (S,L,3).  nan_flag (device uint32, may be NULL) as in gh_project_backward and
+ *   gh_strand_backward.  No head-row and no camera gradients.  S, L > 0.
+ */
+int gh_hair_strands_forward_binned_capturable(
+    int n_head, int S, int L, int width, int height,
+    const float* head_xyz, const float* head_scaling, const float* head_rotation,
+    const float* head_features_dc, const float* head_features_rest, const float* head_opacity,
+    unsigned int head_flags, float head_det_eps,
+    const float* origins, const float* dirs, const float* scale,
+    const float* features_dc, const float* features_rest, const float* orient_conf,
+    unsigned int flags, float det_eps,
+    const float* viewmatrix, const float* projmatrix, const float* campos,
+    const float* tan_fov, float scale_modifier, int sh_degree,
+    float* midpoints,
+    float* means2D, float* colors, float* opacities, float* conic, unsigned char* visible,
+    int* radii, char* geom_buffer, char* img_buffer, char* binning_buffer, long long capacity,
+    unsigned int* status, unsigned int* num_rendered, int debug, gh_stream_t stream);
+int gh_hair_strands_backward_capturable(
+    int n_head, int S, int L, int width, int height,
+    const float* midpoints, const float* dirs, const float* scale,
+    const float* features_dc, const float* features_rest, const float* orient_conf,
+    unsigned int flags, float det_eps,
+    const float* viewmatrix, const float* projmatrix, const float* campos,
+    const float* tan_fov, float scale_modifier, int sh_degree,
+    const unsigned char* visible, const char* geom_buffer,
+    float* d_xyz, float* d_dirs, float* d_features_dc, float* d_features_rest, float* d_orient_conf,
+    unsigned int* nan_flag, int debug, gh_stream_t stream);
+
+/*
  * Trainable cameras (DESIGN §17): the reference's BARF camera model (src/scene/cameras.py:95-152, use_barf = True) and
  * its camera Adam (src/train_gaussians.py:45-63, 183-196).  A rig of n cameras owns, on the device:
  *   base       float[n][18]  C = the float32 _colmap_transform (16, row-major), FoVx, FoVy (the camera's base state)

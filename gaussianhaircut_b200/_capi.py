@@ -136,6 +136,24 @@ SIGNATURES = {
         _p, _p,                              # visible geom_buffer
         _p, _p, _p, _p, _p,                  # d_xyz d_dirs d_features_dc d_features_rest d_orient_conf
         _p, _i, _p]),                        # nan_flag debug stream
+    "gh_hair_segments_forward_binned_capturable": (_i, [
+        _i, _i, _i, _i,                      # n_head N width height
+        _p, _p, _p, _p, _p, _p,              # head: xyz scaling rotation features_dc features_rest opacity
+        C.c_uint, _f,                        # head_flags head_det_eps
+        _p, _p, _p, _p, _p, _p,              # xyz dirs scale features_dc features_rest orient_conf
+        C.c_uint, _f,                        # flags det_eps
+        _p, _p, _p, _p, _f, _i,              # viewmatrix projmatrix campos tan_fov scale_modifier sh_degree
+        _p, _p, _p, _p, _p,                  # means2D colors opacities conic visible
+        _p, _p, _p, _p, _ll,                 # radii geom_buffer img_buffer binning_buffer capacity
+        _p, _p, _i, _p]),                    # status num_rendered debug stream
+    "gh_hair_segments_backward_capturable": (_i, [
+        _i, _i, _i, _i,                      # n_head N width height
+        _p, _p, _p, _p, _p, _p,              # xyz dirs scale features_dc features_rest orient_conf
+        C.c_uint, _f,                        # flags det_eps
+        _p, _p, _p, _p, _f, _i,              # viewmatrix projmatrix campos tan_fov scale_modifier sh_degree
+        _p, _p,                              # visible geom_buffer
+        _p, _p, _p, _p, _p,                  # d_xyz d_dirs d_features_dc d_features_rest d_orient_conf
+        _p, _i, _p]),                        # nan_flag debug stream
     "gh_strand_midpoints": (_i, [_i, _i, _p, _p, _p, _p]),          # S L origins dirs xyz stream
     "gh_strand_backward": (_i, [_i, _i, _p, _p, _p, _p]),           # S L d_xyz d_dirs nan_flag stream
     "gh_densify_classify": (_i, [_i, _p, _p, _p, _p, _f, _f, _f, _f, _p, _p]),

@@ -379,17 +379,29 @@ GhProjArgs gh_proj_args(int P, int width, int height, const float* xyz, const fl
 // flag bit 10: the strand instantiation (Gaussian i = segment i of a polyline, geometry derived from dirs[i])
 bool gh_proj_strand(unsigned int flags) { return (flags >> 10) & 1u; }
 
-// the row counts of the gh_hair_strands_*_capturable entry points: n_head head rows, then S * L segment rows
-int gh_strand_rows_check(const char* who, int n_head, int S, int L, bool need_strands)
+// the row counts of the capturable hair entry points: n_head head rows, then `seg` segment rows; `counts` / `prod` name
+// the segment counts and their product in the messages ("S and L" / "S * L" for polylines, "N" / "N" for given rows)
+int gh_hair_rows_check(const char* who, int n_head, bool negative, unsigned long long seg, bool need_segments,
+                       const char* counts, const char* prod)
 {
     if (n_head < 0) return gh_set_error(GH_E_INVALID_ARG, "%s: n_head must not be negative", who);
-    if (S < 0 || L < 0 || (need_strands && (S == 0 || L == 0)))
-        return gh_set_error(GH_E_INVALID_ARG, "%s: S and L must be %s", who, need_strands ? "positive" : "non-negative");
-    const unsigned long long seg = (unsigned long long)S * (unsigned long long)L;
-    if (3ull * seg > 0x7fffffffull) return gh_set_error(GH_E_INVALID_ARG, "%s: S * L overflows int (3 * S * L must stay below 2^31)", who);
-    if ((unsigned long long)n_head + seg > 0x7fffffffull) return gh_set_error(GH_E_INVALID_ARG, "%s: n_head + S * L overflows int", who);
-    if (n_head == 0 && seg == 0) return gh_set_error(GH_E_INVALID_ARG, "%s: nothing to render (n_head == 0 and S * L == 0)", who);
+    if (negative || (need_segments && seg == 0))
+        return gh_set_error(GH_E_INVALID_ARG, "%s: %s must be %s", who, counts, need_segments ? "positive" : "non-negative");
+    if (3ull * seg > 0x7fffffffull) return gh_set_error(GH_E_INVALID_ARG, "%s: %s overflows int (3 * %s must stay below 2^31)", who, prod, prod);
+    if ((unsigned long long)n_head + seg > 0x7fffffffull) return gh_set_error(GH_E_INVALID_ARG, "%s: n_head + %s overflows int", who, prod);
+    if (n_head == 0 && seg == 0) return gh_set_error(GH_E_INVALID_ARG, "%s: nothing to render (n_head == 0 and %s == 0)", who, prod);
     return GH_OK;
+}
+
+int gh_strand_rows_check(const char* who, int n_head, int S, int L, bool need_strands)
+{
+    return gh_hair_rows_check(who, n_head, S < 0 || L < 0, S < 0 || L < 0 ? 0ull : (unsigned long long)S * (unsigned long long)L,
+                              need_strands, "S and L", "S * L");
+}
+
+int gh_segment_rows_check(const char* who, int n_head, int N, bool need_segments)
+{
+    return gh_hair_rows_check(who, n_head, N < 0, N < 0 ? 0ull : (unsigned long long)N, need_segments, "N", "N");
 }
 
 }  // namespace
@@ -605,10 +617,110 @@ extern "C" int gh_project_backward_capturable(
 }
 
 // ------------------------------------------------------------------------------------------------ capturable, strands
-// The strand model behind its frozen head block (render_hair_strands) in one capturable first phase over P = n_head +
-// S * L rows -- head rows first, then the segments, the row order of the eager path -- and the records-mode parameter
-// backward of the segment rows.  The head block is frozen and the cameras are not trained: no head-row or camera
-// gradients.
+// A segment model behind its frozen head block in one capturable first phase over P = n_head + n_seg rows -- head rows
+// first, then the segments, the row order of the eager path -- and the records-mode parameter backward of the segment
+// rows.  The head block is frozen and the cameras are not trained: no head-row or camera gradients.  Two models share
+// these bodies:
+//  - strands (render_hair_strands): S polylines of L segments from `origins` and `dirs`; the forward computes the
+//    midpoints into `midpoints` first, the backward completes d_dirs with the suffix scan of the cumulative sum;
+//  - segments (render_hair_segments): the n_seg midpoints `xyz` and segment vectors `dirs` as given; no midpoints
+//    kernel and no suffix scan, the two gradients leave as the projection backward writes them.
+// The entry points check the row counts, the capacity and the capturable contract first.
+namespace {
+
+int gh_hair_rows_forward_capturable(
+    const char* who, int n_head, int n_seg, int S, int L, int width, int height,
+    const float* head_xyz, const float* head_scaling, const float* head_rotation,
+    const float* head_features_dc, const float* head_features_rest, const float* head_opacity,
+    unsigned int head_flags, float head_det_eps,
+    const float* origins, float* midpoints, const float* xyz, const float* dirs, const float* scale,
+    const float* features_dc, const float* features_rest, const float* orient_conf,
+    unsigned int flags, float det_eps,
+    const float* viewmatrix, const float* projmatrix, const float* campos,
+    const float* tan_fov, float scale_modifier, int sh_degree,
+    float* means2D, float* colors, float* opacities, float* conic, unsigned char* visible,
+    int* radii, char* geom_buffer, char* img_buffer, char* binning_buffer, long long capacity,
+    unsigned int* status, unsigned int* num_rendered, cudaStream_t stream, bool strands)
+{
+    int rc;
+    if (!tan_fov) return gh_set_error(GH_E_INVALID_ARG, "%s: tan_fov (device float[2]) is required", who);
+    if (!status) return gh_set_error(GH_E_INVALID_ARG, "%s: status (device uint32) is required", who);
+    if (gh_proj_strand(head_flags)) return gh_set_error(GH_E_INVALID_ARG, "%s: head_flags must not set the strand bit", who);
+    if (!gh_proj_strand(flags)) return gh_set_error(GH_E_INVALID_ARG, "%s: flags must set the strand bit (10)", who);
+    const int P = n_head + n_seg;
+    // (the kernels read tan(fov / 2) from tan_fov; 1 stands in for it in the host-side checks)
+    GhProjArgs Ah = gh_proj_args(n_head, width, height, head_xyz, head_scaling, head_rotation, nullptr, head_features_dc,
+                                 head_features_rest, head_opacity, nullptr, nullptr, viewmatrix, projmatrix, campos,
+                                 1.f, 1.f, scale_modifier, sh_degree, head_flags, head_det_eps);
+    GhProjArgs As = gh_proj_args(n_seg, width, height, xyz, scale, nullptr, dirs, features_dc, features_rest, nullptr,
+                                 nullptr, orient_conf, viewmatrix, projmatrix, campos, 1.f, 1.f, scale_modifier, sh_degree,
+                                 flags, det_eps);
+    if (n_head > 0 && (rc = gh_proj_check(Ah, who, false)) != GH_OK) return rc;
+    if (n_seg > 0) {
+        if (strands && (!origins || !midpoints)) return gh_set_error(GH_E_INVALID_ARG, "%s: origins and midpoints are required", who);
+        if ((rc = gh_proj_check(As, who, true)) != GH_OK) return rc;
+    }
+    if (!means2D || !colors || !opacities || !conic || !visible || !radii || !geom_buffer || !img_buffer || !binning_buffer)
+        return gh_set_error(GH_E_INVALID_ARG, "%s: missing output pointer", who);
+    if ((size_t)colors & 7) return gh_set_error(GH_E_INVALID_ARG, "%s: colors must be 8-byte aligned", who);
+    return gh_forward_phase1_capturable(who, P, width, height, radii, geom_buffer, img_buffer, binning_buffer, capacity,
+                                        status, num_rendered, stream, [&](const GhGeomWS& geom, const GhImgWS& img, int gx, int gy) {
+        if (n_head > 0) {
+            gh_project_forward_tan_kernel<<<(n_head + GH_PJ_THREADS - 1) / GH_PJ_THREADS, GH_PJ_THREADS, 0, stream>>>(
+                Ah, tan_fov, means2D, colors, opacities, conic, visible, radii, geom.geo, geom.depth, img.tile_count, gx, gy);
+            gh_count_launches(1);
+        }
+        if (n_seg > 0) {
+            // strands: the midpoints in segment order (bit-identical to the eager path's) into As.xyz = midpoints first;
+            // then the segment rows behind the head's
+            if (strands) {
+                gh_launch_strand_midpoints(S, L, origins, dirs, midpoints, stream);
+                gh_count_launches(1);
+            }
+            const size_t h = (size_t)n_head;
+            gh_project_forward_strand_tan_kernel<<<(n_seg + GH_PJ_THREADS - 1) / GH_PJ_THREADS, GH_PJ_THREADS, 0, stream>>>(
+                As, tan_fov, means2D + 3 * h, colors + GH_NUM_CHANNELS * h, opacities + h, conic + 3 * h, visible + h,
+                radii + h, geom.geo + h, geom.depth + h, img.tile_count, gx, gy);
+            gh_count_launches(1);
+        }
+    });
+}
+
+int gh_hair_rows_backward_capturable(
+    const char* who, int n_head, int n_seg, int S, int L, int width, int height,
+    const float* xyz, const float* dirs, const float* scale,
+    const float* features_dc, const float* features_rest, const float* orient_conf,
+    unsigned int flags, float det_eps,
+    const float* viewmatrix, const float* projmatrix, const float* campos,
+    const float* tan_fov, float scale_modifier, int sh_degree,
+    const unsigned char* visible, const char* geom_buffer,
+    float* d_xyz, float* d_dirs, float* d_features_dc, float* d_features_rest, float* d_orient_conf,
+    unsigned int* nan_flag, cudaStream_t stream, bool strands)
+{
+    if (!tan_fov) return gh_set_error(GH_E_INVALID_ARG, "%s: tan_fov (device float[2]) is required", who);
+    if (!gh_proj_strand(flags)) return gh_set_error(GH_E_INVALID_ARG, "%s: flags must set the strand bit (10)", who);
+    GhProjArgs A = gh_proj_args(n_seg, width, height, xyz, scale, nullptr, dirs, features_dc, features_rest, nullptr,
+                                nullptr, orient_conf, viewmatrix, projmatrix, campos, 1.f, 1.f, scale_modifier, sh_degree,
+                                flags, det_eps);
+    const int rc = gh_proj_check(A, who, true);
+    if (rc != GH_OK) return rc;
+    if (!visible || !geom_buffer || !d_xyz || !d_dirs || !d_features_dc || !d_features_rest)
+        return gh_set_error(GH_E_INVALID_ARG, "%s: missing mandatory pointer", who);
+    // the blend backward's accumulation records of the segment rows, in the geometry workspace of all P rows
+    const size_t h = (size_t)n_head;
+    const float* acc16 = GhGeomWS::carve(const_cast<char*>(geom_buffer), h + (size_t)n_seg).acc16 + 16 * h;
+    gh_project_backward_tan_kernel<true><<<(n_seg + GH_PJ_THREADS - 1) / GH_PJ_THREADS, GH_PJ_THREADS, 0, stream>>>(
+        A, tan_fov, visible + h, acc16, nullptr, nullptr, nullptr, nullptr,
+        d_xyz, nullptr, nullptr, d_dirs, d_features_dc, d_features_rest, nullptr, nullptr, d_orient_conf,
+        nullptr, nullptr, nullptr, nullptr, nan_flag);
+    if (!strands) return gh_launch_status(who, 1);
+    // strands: dL/d midpoint through the cumulative sum into d_dirs
+    gh_launch_strand_backward(S, L, d_xyz, d_dirs, nan_flag, stream);
+    return gh_launch_status(who, 2);
+}
+
+}  // namespace
+
 extern "C" int gh_hair_strands_forward_binned_capturable(
     int n_head, int S, int L, int width, int height,
     const float* head_xyz, const float* head_scaling, const float* head_rotation,
@@ -625,49 +737,17 @@ extern "C" int gh_hair_strands_forward_binned_capturable(
     unsigned int* status, unsigned int* num_rendered, int debug, gh_stream_t stream_)
 {
     const char* who = "gh_hair_strands_forward_binned_capturable";
-    cudaStream_t stream = (cudaStream_t)stream_;
     gh_clear_error();
     int rc = gh_check_capturable(who, debug);
     if (rc == GH_OK) rc = gh_check_capacity(who, capacity);
     if (rc == GH_OK) rc = gh_strand_rows_check(who, n_head, S, L, false);
     if (rc != GH_OK) return rc;
-    if (!tan_fov) return gh_set_error(GH_E_INVALID_ARG, "%s: tan_fov (device float[2]) is required", who);
-    if (!status) return gh_set_error(GH_E_INVALID_ARG, "%s: status (device uint32) is required", who);
-    if (gh_proj_strand(head_flags)) return gh_set_error(GH_E_INVALID_ARG, "%s: head_flags must not set the strand bit", who);
-    if (!gh_proj_strand(flags)) return gh_set_error(GH_E_INVALID_ARG, "%s: flags must set the strand bit (10)", who);
-    const int n_seg = S * L, P = n_head + n_seg;
-    // (the kernels read tan(fov / 2) from tan_fov; 1 stands in for it in the host-side checks)
-    GhProjArgs Ah = gh_proj_args(n_head, width, height, head_xyz, head_scaling, head_rotation, nullptr, head_features_dc,
-                                 head_features_rest, head_opacity, nullptr, nullptr, viewmatrix, projmatrix, campos,
-                                 1.f, 1.f, scale_modifier, sh_degree, head_flags, head_det_eps);
-    GhProjArgs As = gh_proj_args(n_seg, width, height, midpoints, scale, nullptr, dirs, features_dc, features_rest, nullptr,
-                                 nullptr, orient_conf, viewmatrix, projmatrix, campos, 1.f, 1.f, scale_modifier, sh_degree,
-                                 flags, det_eps);
-    if (n_head > 0 && (rc = gh_proj_check(Ah, who, false)) != GH_OK) return rc;
-    if (n_seg > 0) {
-        if (!origins || !midpoints) return gh_set_error(GH_E_INVALID_ARG, "%s: origins and midpoints are required", who);
-        if ((rc = gh_proj_check(As, who, true)) != GH_OK) return rc;
-    }
-    if (!means2D || !colors || !opacities || !conic || !visible || !radii || !geom_buffer || !img_buffer || !binning_buffer)
-        return gh_set_error(GH_E_INVALID_ARG, "%s: missing output pointer", who);
-    if ((size_t)colors & 7) return gh_set_error(GH_E_INVALID_ARG, "%s: colors must be 8-byte aligned", who);
-    return gh_forward_phase1_capturable(who, P, width, height, radii, geom_buffer, img_buffer, binning_buffer, capacity,
-                                        status, num_rendered, stream, [&](const GhGeomWS& geom, const GhImgWS& img, int gx, int gy) {
-        if (n_head > 0) {
-            gh_project_forward_tan_kernel<<<(n_head + GH_PJ_THREADS - 1) / GH_PJ_THREADS, GH_PJ_THREADS, 0, stream>>>(
-                Ah, tan_fov, means2D, colors, opacities, conic, visible, radii, geom.geo, geom.depth, img.tile_count, gx, gy);
-            gh_count_launches(1);
-        }
-        if (n_seg > 0) {
-            // the midpoints in segment order (bit-identical to the eager path's), then the segment rows behind the head's
-            gh_launch_strand_midpoints(S, L, origins, dirs, midpoints, stream);
-            const size_t h = (size_t)n_head;
-            gh_project_forward_strand_tan_kernel<<<(n_seg + GH_PJ_THREADS - 1) / GH_PJ_THREADS, GH_PJ_THREADS, 0, stream>>>(
-                As, tan_fov, means2D + 3 * h, colors + GH_NUM_CHANNELS * h, opacities + h, conic + 3 * h, visible + h,
-                radii + h, geom.geo + h, geom.depth + h, img.tile_count, gx, gy);
-            gh_count_launches(2);
-        }
-    });
+    return gh_hair_rows_forward_capturable(
+        who, n_head, S * L, S, L, width, height, head_xyz, head_scaling, head_rotation, head_features_dc,
+        head_features_rest, head_opacity, head_flags, head_det_eps, origins, midpoints, midpoints, dirs, scale, features_dc,
+        features_rest, orient_conf, flags, det_eps, viewmatrix, projmatrix, campos, tan_fov, scale_modifier, sh_degree,
+        means2D, colors, opacities, conic, visible, radii, geom_buffer, img_buffer, binning_buffer, capacity, status,
+        num_rendered, (cudaStream_t)stream_, true);
 }
 
 extern "C" int gh_hair_strands_backward_capturable(
@@ -682,28 +762,67 @@ extern "C" int gh_hair_strands_backward_capturable(
     unsigned int* nan_flag, int debug, gh_stream_t stream_)
 {
     const char* who = "gh_hair_strands_backward_capturable";
-    cudaStream_t stream = (cudaStream_t)stream_;
     gh_clear_error();
     int rc = gh_check_capturable(who, debug);
     if (rc == GH_OK) rc = gh_strand_rows_check(who, n_head, S, L, true);
     if (rc != GH_OK) return rc;
-    if (!tan_fov) return gh_set_error(GH_E_INVALID_ARG, "%s: tan_fov (device float[2]) is required", who);
-    if (!gh_proj_strand(flags)) return gh_set_error(GH_E_INVALID_ARG, "%s: flags must set the strand bit (10)", who);
-    const int n_seg = S * L;
-    GhProjArgs A = gh_proj_args(n_seg, width, height, midpoints, scale, nullptr, dirs, features_dc, features_rest, nullptr,
-                                nullptr, orient_conf, viewmatrix, projmatrix, campos, 1.f, 1.f, scale_modifier, sh_degree,
-                                flags, det_eps);
-    rc = gh_proj_check(A, who, true);
+    return gh_hair_rows_backward_capturable(
+        who, n_head, S * L, S, L, width, height, midpoints, dirs, scale, features_dc, features_rest, orient_conf, flags,
+        det_eps, viewmatrix, projmatrix, campos, tan_fov, scale_modifier, sh_degree, visible, geom_buffer, d_xyz, d_dirs,
+        d_features_dc, d_features_rest, d_orient_conf, nan_flag, (cudaStream_t)stream_, true);
+}
+
+// ------------------------------------------------------------------------------------------------ capturable, segments
+// The latent strand model (render_hair_segments): its N segment rows come as given midpoints `xyz` and segment vectors
+// `dirs` (what GaussianModelHair.generate_strands leaves in _xyz and _dir), not as polylines.
+extern "C" int gh_hair_segments_forward_binned_capturable(
+    int n_head, int N, int width, int height,
+    const float* head_xyz, const float* head_scaling, const float* head_rotation,
+    const float* head_features_dc, const float* head_features_rest, const float* head_opacity,
+    unsigned int head_flags, float head_det_eps,
+    const float* xyz, const float* dirs, const float* scale,
+    const float* features_dc, const float* features_rest, const float* orient_conf,
+    unsigned int flags, float det_eps,
+    const float* viewmatrix, const float* projmatrix, const float* campos,
+    const float* tan_fov, float scale_modifier, int sh_degree,
+    float* means2D, float* colors, float* opacities, float* conic, unsigned char* visible,
+    int* radii, char* geom_buffer, char* img_buffer, char* binning_buffer, long long capacity,
+    unsigned int* status, unsigned int* num_rendered, int debug, gh_stream_t stream_)
+{
+    const char* who = "gh_hair_segments_forward_binned_capturable";
+    gh_clear_error();
+    int rc = gh_check_capturable(who, debug);
+    if (rc == GH_OK) rc = gh_check_capacity(who, capacity);
+    if (rc == GH_OK) rc = gh_segment_rows_check(who, n_head, N, false);
     if (rc != GH_OK) return rc;
-    if (!visible || !geom_buffer || !d_xyz || !d_dirs || !d_features_dc || !d_features_rest)
-        return gh_set_error(GH_E_INVALID_ARG, "%s: missing mandatory pointer", who);
-    // the blend backward's accumulation records of the segment rows, in the geometry workspace of all P rows
-    const size_t h = (size_t)n_head;
-    const float* acc16 = GhGeomWS::carve(const_cast<char*>(geom_buffer), h + (size_t)n_seg).acc16 + 16 * h;
-    gh_project_backward_tan_kernel<true><<<(n_seg + GH_PJ_THREADS - 1) / GH_PJ_THREADS, GH_PJ_THREADS, 0, stream>>>(
-        A, tan_fov, visible + h, acc16, nullptr, nullptr, nullptr, nullptr,
-        d_xyz, nullptr, nullptr, d_dirs, d_features_dc, d_features_rest, nullptr, nullptr, d_orient_conf,
-        nullptr, nullptr, nullptr, nullptr, nan_flag);
-    gh_launch_strand_backward(S, L, d_xyz, d_dirs, nan_flag, stream);
-    return gh_launch_status(who, 2);
+    if (!xyz || !dirs) return gh_set_error(GH_E_INVALID_ARG, "%s: xyz and dirs (the segment rows) are required", who);
+    return gh_hair_rows_forward_capturable(
+        who, n_head, N, 0, 0, width, height, head_xyz, head_scaling, head_rotation, head_features_dc, head_features_rest,
+        head_opacity, head_flags, head_det_eps, nullptr, nullptr, xyz, dirs, scale, features_dc, features_rest, orient_conf,
+        flags, det_eps, viewmatrix, projmatrix, campos, tan_fov, scale_modifier, sh_degree, means2D, colors, opacities,
+        conic, visible, radii, geom_buffer, img_buffer, binning_buffer, capacity, status, num_rendered,
+        (cudaStream_t)stream_, false);
+}
+
+extern "C" int gh_hair_segments_backward_capturable(
+    int n_head, int N, int width, int height,
+    const float* xyz, const float* dirs, const float* scale,
+    const float* features_dc, const float* features_rest, const float* orient_conf,
+    unsigned int flags, float det_eps,
+    const float* viewmatrix, const float* projmatrix, const float* campos,
+    const float* tan_fov, float scale_modifier, int sh_degree,
+    const unsigned char* visible, const char* geom_buffer,
+    float* d_xyz, float* d_dirs, float* d_features_dc, float* d_features_rest, float* d_orient_conf,
+    unsigned int* nan_flag, int debug, gh_stream_t stream_)
+{
+    const char* who = "gh_hair_segments_backward_capturable";
+    gh_clear_error();
+    int rc = gh_check_capturable(who, debug);
+    if (rc == GH_OK) rc = gh_segment_rows_check(who, n_head, N, true);
+    if (rc != GH_OK) return rc;
+    if (!xyz || !dirs) return gh_set_error(GH_E_INVALID_ARG, "%s: xyz and dirs (the segment rows) are required", who);
+    return gh_hair_rows_backward_capturable(
+        who, n_head, N, 0, 0, width, height, xyz, dirs, scale, features_dc, features_rest, orient_conf, flags, det_eps,
+        viewmatrix, projmatrix, campos, tan_fov, scale_modifier, sh_degree, visible, geom_buffer, d_xyz, d_dirs,
+        d_features_dc, d_features_rest, d_orient_conf, nan_flag, (cudaStream_t)stream_, false);
 }

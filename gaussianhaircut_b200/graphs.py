@@ -25,8 +25,13 @@ render_hair_strands_capturable (frozen head block + strand model) -> strand_imag
 `_dirs` gradient, computed outside the graph) -> FusedAdam.  The two classes share the warm-up on a side stream, the
 capacity seeding, the overflow rerun and recapture, and the pinned read-back (_CapturedStep).
 
-Not captured: render_hair (train_latent_strands.py: its strands come from networks outside this package), the
-multi-GPU gradient all-reduce (gh_allreduce_p2p takes its epoch as a host argument).
+`CapturedLatentStrandStep.step()` captures the part of the `src/train_latent_strands.py` iteration that runs in this
+package (DESIGN §20): render_hair_segments_capturable (frozen head block + the decoder's segment rows) ->
+latent_strand_image_loss -> backward into static gradients of the five decoder outputs.  The strand networks, their
+prior term and their AdamW stay eager, outside the graph: step() returns a loss tensor whose backward hands the static
+gradients to them.
+
+Not captured: the multi-GPU gradient all-reduce (gh_allreduce_p2p takes its epoch as a host argument).
 """
 from __future__ import annotations
 
@@ -40,8 +45,8 @@ from ._C import capacity_for
 from .cameras import CameraAdam, CameraView, STATUS_CAMERA_INDEX
 from .optim import FusedAdam
 
-__all__ = ["CapturedTrainStep", "CapturedStrandStep", "capture_key", "strand_capture_key", "check_dirs_grad", "capacity_for",
-           "STATUS_BINNING_OVERFLOW", "STATUS_CAMERA_INDEX"]
+__all__ = ["CapturedTrainStep", "CapturedStrandStep", "CapturedLatentStrandStep", "capture_key", "strand_capture_key",
+           "latent_capture_key", "check_dirs_grad", "capacity_for", "STATUS_BINNING_OVERFLOW", "STATUS_CAMERA_INDEX"]
 
 STATUS_BINNING_OVERFLOW = 1      # GH_STATUS_BINNING_OVERFLOW
 WARMUP_ITERS = 2                 # eager iterations (on a side stream) before each capture
@@ -103,6 +108,25 @@ def strand_capture_key(pc, pc_hair, optimizer, width: int, height: int, use_gt_o
             bool(dirs_grad), tuple(ptrs), head_ptrs, cam)
 
 
+def latent_capture_key(pc, pc_hair, width: int, height: int, use_gt_orient_conf: bool = True,
+                       train_orient_conf: bool = True, cameras=None) -> tuple:
+    """What a captured latent strand iteration is specialised to: the segment rows N, the head block's size n_head,
+    the image size, the strand model's active SH degree, torch.are_deterministic_algorithms_enabled(), the two loss
+    options, and the storage of `scale`, of the cached head block (renderer._head_block) and of the rig's tables when
+    views of a cameras.CameraRig are rendered.  The decoder's outputs are copied into buffers the step owns, so their
+    storage is not part of the key.  A different key means a new capture."""
+    N = int(pc_hair._xyz.shape[0])
+    head = renderer._head_block(pc) if pc is not None else None
+    n_head = 0 if head is None else int(head["xyz"].shape[0])
+    head_ptrs = () if head is None else tuple(head[k].data_ptr() for k in ("xyz", "scaling", "rotation", "opacity",
+                                                                            "f_dc", "f_rest"))
+    scale = pc_hair.scale
+    cam = _rig_tables(cameras) if cameras is not None else ()
+    return (N, n_head, int(width), int(height), int(pc_hair.active_sh_degree),
+            bool(torch.are_deterministic_algorithms_enabled()), bool(use_gt_orient_conf), bool(train_orient_conf),
+            scale.data_ptr() if isinstance(scale, torch.Tensor) else 0, head_ptrs, cam)
+
+
 def check_dirs_grad(dirs_grad: torch.Tensor, dirs: torch.Tensor) -> None:
     """The prior gradient a strand trainer hands to CapturedStrandStep.step(): float32, on the device of `_dirs`, and
     of its (S, L, 3) shape."""
@@ -146,11 +170,14 @@ class _CapturedStep:
     replay that falls back to the eager iteration on a binning overflow."""
 
     def __init__(self, who: str, optimizer, width: int, height: int, bg: torch.Tensor, lambdas: Sequence[float],
-                 capacity: Optional[int], pipe, device):
+                 capacity: Optional[int], pipe, device, needs_optimizer: bool = True):
+        """`needs_optimizer=False`: the iteration has no optimizer inside the graph (`optimizer` must then be None)."""
         if getattr(pipe, "debug", False):
             raise RuntimeError(f"{who}: debug mode synchronises after every stage and cannot be captured")
-        if not isinstance(optimizer, FusedAdam) or not optimizer.capturable:
+        if needs_optimizer and (not isinstance(optimizer, FusedAdam) or not optimizer.capturable):
             raise RuntimeError(f"{who} needs FusedAdam(..., capturable=True)")
+        if not needs_optimizer and optimizer is not None:
+            raise RuntimeError(f"{who}: the iteration has no optimizer inside the graph")
         _check_no_arena(who)
         self.optimizer = optimizer
         self.W, self.H = int(width), int(height)
@@ -204,7 +231,8 @@ class _CapturedStep:
         self.capacity = max(self.capacity, capacity_for(self.r_max))
         self._graph = None
         self._binning = _C.binning_workspace(self.capacity, self.device)
-        self.optimizer.zero_grad(set_to_none=True)
+        if self.optimizer is not None:
+            self.optimizer.zero_grad(set_to_none=True)
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g):
             self._with_nan_flag(captured)
@@ -491,3 +519,168 @@ class CapturedStrandStep(_CapturedStep):
                              lambda: self._captured(rig_view, static_dirs_grad),
                              lambda: self._load(camera, gts, rig_view, dirs_grad, static_dirs_grad),
                              "CapturedStrandStep")
+
+
+SEGMENT_TENSORS = ("_xyz", "_dir", "_features_dc", "_features_rest", "_orient_conf")
+
+
+class _StaticGradients(torch.autograd.Function):
+    """(total, step, generation, xyz, dirs, f_dc, f_rest, conf) -> the 0-dim image loss of one CapturedLatentStrandStep
+    step, connected to the five decoder outputs: the backward returns grad_output times the step's gradients (exact
+    for grad_output = 1), and raises when a later step has overwritten them."""
+
+    @staticmethod
+    def forward(ctx, total, step, generation, *tensors):
+        ctx.step, ctx.generation = step, generation
+        return total.clone()
+
+    @staticmethod
+    def backward(ctx, g):
+        step = ctx.step
+        if ctx.generation != step._generation or step._grads is None:
+            raise RuntimeError(f"CapturedLatentStrandStep: this loss is from step {ctx.generation}, but its gradients "
+                               f"were overwritten by step {step._generation}; call backward() before the next step()")
+        need = ctx.needs_input_grad
+        return (None, None, None) + tuple(gr * g if need[3 + i] else None for i, gr in enumerate(step._grads))
+
+
+class CapturedLatentStrandStep(_CapturedStep):
+    """The render, loss and backward of one `train_latent_strands.py` iteration per `step()`, replayed from a CUDA
+    graph (DESIGN §20).  The strand networks stay outside the graph: the trainer runs their forward
+    (`pc_hair.generate_strands(iteration)`), hands the model to step(), adds its prior term to the returned loss,
+    calls backward() and steps its AdamW.
+
+    pc: the frozen head GaussianModel with the trainer's *_precomp attributes (renderer._head_block), or None for a
+      hair-only model; bg: the (10,) background; lambdas: (l1, mask, orient) loss weights (opt.lambda_dl1,
+      lambda_dmask, lambda_dorient); use_gt_orient_conf / train_orient_conf: the trainer's options of
+      latent_strand_image_loss; capacity: the initial binning capacity in records (None: seeded from the warm-up
+      iterations); pipe: the trainer's pipeline options (`debug` must be off); cameras: a cameras.CameraRig whose
+      frozen views step() receives (None: cameras are plain objects with fixed tensors).
+
+    The eager iteration (warm-ups and overflow reruns) is render_hair_segments -> image_loss_forward_backward(stage=
+    "latent_strands") -> backward; the captured one computes the same values (bit for bit under
+    torch.use_deterministic_algorithms(True)).  Both end in the same gradient contract.
+    """
+
+    def __init__(self, pc, width: int, height: int, bg: torch.Tensor, lambdas: Sequence[float],
+                 use_gt_orient_conf: bool = True, train_orient_conf: bool = True, capacity: Optional[int] = None,
+                 pipe=None, cameras=None):
+        if len(lambdas) != 3:
+            raise RuntimeError("CapturedLatentStrandStep: lambdas are (l1, mask, orient)")
+        super().__init__("CapturedLatentStrandStep", None, width, height, bg, lambdas, capacity, pipe, bg.device,
+                         needs_optimizer=False)
+        self.pc, self.cameras = pc, cameras
+        self.use_gt_orient_conf, self.train_orient_conf = bool(use_gt_orient_conf), bool(train_orient_conf)
+        self._cam_out = torch.zeros(37, dtype=torch.float32, device=self.device)
+        self._inputs = None             # the static copies of the five decoder outputs (leaves of the captured render)
+        self._static_grads = None       # their gradients, written by every replay
+        self._grads = None              # the gradients of the latest step (static or eager)
+        self._generation = 0
+
+    # ------------------------------------------------------------------------------------------ the iteration
+    def _tail(self, renders, gts):
+        """loss -> backward, shared by the eager and the captured iteration; the 8 losses land in the static words."""
+        l1, lmask, lorient = self.lambdas          # (latent_strand_image_loss: no SSIM term)
+        losses8, dL = ghl.image_loss_forward_backward(renders.detach(), *gts, l1, 0.0, lmask, lorient, workspace=self._ws,
+                                                      stage="latent_strands", use_gt_orient_conf=self.use_gt_orient_conf,
+                                                      train_orient_conf=self.train_orient_conf)
+        renders.backward(dL)
+        self._io[2:].copy_(losses8.view(torch.int32))
+        return losses8
+
+    def _model(self, pc_hair, tensors):
+        return types.SimpleNamespace(scale=pc_hair.scale, active_sh_degree=pc_hair.active_sh_degree,
+                                     **dict(zip(SEGMENT_TENSORS, tensors)))
+
+    def _eager(self, camera, gts, pc_hair) -> torch.Tensor:
+        """The eager iteration (renderer.render_hair_segments) on a side stream, on leaves that share the decoder
+        outputs' storage.  A rig view is rendered frozen."""
+        leaves = [getattr(pc_hair, n).detach().requires_grad_(True) for n in SEGMENT_TENSORS]
+
+        def run():
+            cam = camera
+            if isinstance(cam, CameraView):
+                cam = cam.rig.view(cam.index, requires_grad=False)
+            pkg = renderer.render_hair_segments(cam, self.pc, self._model(pc_hair, leaves), self.pipe, self.bg)
+            return self._with_nan_flag(lambda: self._tail(pkg["raw"], gts))
+
+        losses8 = _on_side_stream(self.device, run)
+        self._grads = tuple(t.grad for t in leaves)
+        self._record_r(self._rows(pc_hair))
+        return losses8.cpu()
+
+    def _rows(self, pc_hair) -> int:
+        head = renderer._head_block(self.pc) if self.pc is not None else None
+        return (0 if head is None else int(head["xyz"].shape[0])) + int(pc_hair._xyz.shape[0])
+
+    def _captured(self, rig_view: bool, pc_hair):
+        status, n_rendered = self._io[0:1], self._io[1:2]
+        status.zero_()
+        camera = self._camera
+        if rig_view:
+            out = self._cam_out
+            self.cameras.forward(self._cam_index, out=out, status=status)
+            camera = {"viewmatrix": out[0:16].view(4, 4), "projmatrix": out[16:32].view(4, 4), "campos": out[32:35],
+                      "tan_fov": out[35:37]}
+        for t in self._inputs:
+            t.grad = None
+        renders, _radii = renderer.render_hair_segments_capturable(camera, self.pc, self._model(pc_hair, self._inputs),
+                                                                   self.bg, self.W, self.H, self._binning, self.capacity,
+                                                                   status, n_rendered)
+        self._tail(renders, self._gt)
+        self._static_grads = tuple(t.grad for t in self._inputs)
+
+    def _static_inputs(self, tensors) -> None:
+        """The step's own copies of the decoder outputs, reallocated (and the graph dropped) when a shape changes."""
+        shapes = tuple(tuple(t.shape) for t in tensors)
+        if self._inputs is None or tuple(tuple(t.shape) for t in self._inputs) != shapes:
+            self._inputs = tuple(torch.zeros(sh, dtype=torch.float32, device=self.device, requires_grad=True)
+                                 for sh in shapes)
+            self._static_grads = None
+            self._graph, self._binning, self._key = None, None, None
+
+    def _load(self, camera, gts, rig_view: bool, tensors) -> None:
+        if rig_view:
+            self._cam_index.copy_(camera.rig.indices[camera.index:camera.index + 1])
+        else:
+            self._load_camera(camera)
+        for dst, src in zip(self._gt, gts):
+            if src is not None:
+                dst.copy_(src)
+        with torch.no_grad():
+            for dst, src in zip(self._inputs, tensors):
+                dst.copy_(src)
+        self._grads = self._static_grads
+
+    # ------------------------------------------------------------------------------------------ public
+    def step(self, camera, gt_image, gt_mask, gt_orient_angle, gt_orient_conf, pc_hair):
+        """Render, loss and backward of one iteration on `camera` for the segment rows `pc_hair` holds now (after
+        `generate_strands`: `_xyz`, `_dir`, `_features_dc`, `_features_rest`, `_orient_conf`, `scale` a (1,) device
+        tensor, `active_sh_degree`) -> (loss, losses).  `loss`: the 0-dim total of the image terms on the device,
+        connected to the five tensors -- its backward adds grad_output times their gradients, which stay valid until
+        the next step() (a backward after it raises); `losses`: the eight losses of latent_strand_image_loss (float32
+        CPU tensor: total, Ll1, 0, LCE, LOR, sum of orientation weights, LOR-was-NaN, the other replaced terms).
+        `camera`: a (frozen) view of `cameras` or a camera with fixed tensors."""
+        self._generation += 1
+        self._grads = None
+        rig_view = self.cameras is not None and isinstance(camera, CameraView) and camera.rig is self.cameras
+        if not rig_view:
+            _check_camera(camera, "CapturedLatentStrandStep", "renderer.render_hair_segments")
+        _check_no_arena("CapturedLatentStrandStep")
+        if not isinstance(pc_hair.scale, torch.Tensor):
+            raise RuntimeError("CapturedLatentStrandStep: pc_hair.scale must be a (1,) device tensor")
+        if renderer._segment_rows(pc_hair, "CapturedLatentStrandStep") < 1:
+            raise RuntimeError("CapturedLatentStrandStep: the model has no segment rows")
+        if gt_orient_conf is None and self.use_gt_orient_conf:
+            raise RuntimeError("CapturedLatentStrandStep: gt_orient_conf is required with use_gt_orient_conf=True")
+        tensors = tuple(getattr(pc_hair, n) for n in SEGMENT_TENSORS)
+        self._static_inputs(tensors)
+        gts = (gt_image, gt_mask, gt_orient_angle, gt_orient_conf)
+        losses8 = self._iterate(lambda: latent_capture_key(self.pc, pc_hair, self.W, self.H, self.use_gt_orient_conf,
+                                                           self.train_orient_conf, self.cameras if rig_view else None),
+                                lambda: self._eager(camera, gts, pc_hair),
+                                lambda: self._captured(rig_view, pc_hair),
+                                lambda: self._load(camera, gts, rig_view, tensors),
+                                "CapturedLatentStrandStep")
+        total = self._io[2:3].view(torch.float32).reshape(())
+        return _StaticGradients.apply(total, self, self._generation, *tensors), losses8

@@ -408,3 +408,93 @@ def hair_strands_backward_capturable(sp: StrandInputs, midpoints: torch.Tensor, 
     g["dirs"] = g["dirs"].view(sp.S, sp.L, 3)
     del g["xyz"]
     return g
+
+
+# ------------------------------------------------------------------------------------------------ capturable segments
+class SegmentInputs:
+    """The (detached, contiguous) tensors of one capturable segment render (head block + the latent strand model's N
+    given segment rows), kept between the forward and the backward."""
+    __slots__ = ("n_head", "N", "W", "H", "head", "xyz", "dirs", "scale", "f_dc", "f_rest", "conf", "V", "Pm", "campos",
+                 "tan_fov", "mod", "sh_degree", "device")
+
+    @property
+    def P(self) -> int:
+        return self.n_head + self.N
+
+    def common(self):
+        """The arguments shared by the two gh_hair_segments_*_capturable entry points after the image size."""
+        return (_ptr(self.xyz), _ptr(self.dirs), _ptr(self.scale), _ptr(self.f_dc), _ptr(self.f_rest), _ptr(self.conf),
+                encode_flags(HAIR_STRANDS), float(HAIR_STRANDS["det_eps"]), _ptr(self.V), _ptr(self.Pm), _ptr(self.campos),
+                _ptr(self.tan_fov), self.mod, self.sh_degree)
+
+
+def pack_segment_inputs(head, xyz, dirs, scale, f_dc, f_rest, conf, viewmatrix, projmatrix, campos, tan_fov,
+                        width: int, height: int, sh_degree: int, scaling_modifier: float) -> SegmentInputs:
+    """`head`: the frozen head block (renderer._head_block) or None; `xyz` (N,3) segment midpoints and `dirs` (N,3)
+    segment vectors (GaussianModelHair._xyz / _dir), `scale` the (1,) strand thickness, f_dc / f_rest / conf with N
+    rows; the camera tensors and the (2,) `tan_fov` on the device."""
+    dev = xyz.device
+    if xyz.ndim != 2 or xyz.shape[-1] != 3 or tuple(dirs.shape) != tuple(xyz.shape):
+        raise RuntimeError(f"projection: xyz and dirs must both be (N, 3), got {tuple(xyz.shape)} and {tuple(dirs.shape)}")
+    sp = SegmentInputs()
+    sp.device = dev
+    sp.N, sp.W, sp.H = int(xyz.shape[0]), int(width), int(height)
+    sp.head = None
+    if head is not None and int(head["xyz"].shape[0]) > 0:
+        sp.head = {k: _f32(head[k], "head " + k, dev, align=16 if k == "rotation" else 4)
+                   for k in ("xyz", "scaling", "rotation", "f_dc", "f_rest", "opacity")}
+    sp.n_head = 0 if sp.head is None else int(sp.head["xyz"].shape[0])
+    sp.xyz, sp.dirs, sp.scale = _f32(xyz, "xyz", dev), _f32(dirs, "dirs", dev), _f32(scale, "scale", dev)
+    sp.f_dc, sp.f_rest, sp.conf = _f32(f_dc, "features_dc", dev), _f32(f_rest, "features_rest", dev), _f32(conf, "orient_conf", dev)
+    sp.V, sp.Pm, sp.campos = _f32(viewmatrix, "viewmatrix", dev), _f32(projmatrix, "projmatrix", dev), _f32(campos, "campos", dev)
+    sp.tan_fov = _f32(tan_fov, "tan_fov", dev)
+    sp.mod, sp.sh_degree = float(scaling_modifier), int(sh_degree)
+    n = sp.N
+    if sp.scale is None or sp.scale.numel() != 1:
+        raise RuntimeError("projection: the strand thickness must be a (1,) tensor")
+    for name, t, per in (("features_dc", sp.f_dc, 3), ("orient_conf", sp.conf, 1)):
+        if t is None or t.numel() != n * per:
+            raise RuntimeError(f"projection: '{name}' must have {per} floats per segment (N = {n} rows)")
+    if sp.sh_degree > 0 and (sp.f_rest is None or sp.f_rest.numel() != n * 45):
+        raise RuntimeError("projection: 'features_rest' must be (N, 15, 3) for sh_degree > 0")
+    return sp
+
+
+def hair_segments_forward_binned_capturable(sp: SegmentInputs, binning: torch.Tensor, capacity: int,
+                                            status: torch.Tensor, num_rendered: Optional[torch.Tensor] = None):
+    """gh_hair_segments_forward_binned_capturable: the capturable first phase of render_hair_segments over P = n_head +
+    N rows (head rows first).  -> (out dict as project_forward with P rows, radii, geomBuffer, imgBuffer); continue
+    with `_C.forward_render_capturable`.  No host synchronisation."""
+    from . import _C
+    lib = _capi.load()
+    dev, P = sp.device, sp.P
+    out = alloc_outputs(P, dev)
+    geom, img, radii = _C.alloc_forward_workspaces(P, sp.W, sp.H, dev)
+    hd = sp.head or {}
+    h = lambda k: _ptr(hd.get(k))  # noqa: E731
+    with torch.cuda.device(dev):
+        _capi.check(lib.gh_hair_segments_forward_binned_capturable(
+            sp.n_head, sp.N, sp.W, sp.H, h("xyz"), h("scaling"), h("rotation"), h("f_dc"), h("f_rest"), h("opacity"),
+            encode_flags(HEAD_PRECOMP), float(HEAD_PRECOMP["det_eps"]), *sp.common(),
+            _ptr(out["means2D"]), _ptr(out["colors"]), _ptr(out["opacity"]), _ptr(out["conic"]), _ptr(out["visible"]),
+            _ptr(radii), _ptr(geom), _ptr(img), _ptr(binning), int(capacity), _ptr(status), _ptr(num_rendered), 0,
+            _stream(dev)))
+    return out, radii, geom, img
+
+
+def hair_segments_backward_capturable(sp: SegmentInputs, visible: torch.Tensor, geom_buffer: torch.Tensor,
+                                      nan_flag: Optional[torch.Tensor] = None):
+    """gh_hair_segments_backward_capturable, after `_C.backward_records_capturable` over all P rows: the gradients of
+    the segment rows from their accumulation records -> dict(xyz (N,3), dirs (N,3), f_dc (N,1,3), f_rest (N,15,3),
+    conf (N,1)).  `nan_flag` as in project_backward."""
+    _check_no_strand_arena()
+    lib = _capi.load()
+    dev, n = sp.device, sp.N
+    g = {k: empty_rows(n, shape, torch.float32, dev) for k, shape in (("xyz", (3,)), ("dirs", (3,)), ("f_dc", (1, 3)),
+                                                                      ("f_rest", (15, 3)), ("conf", (1,)))}
+    with torch.cuda.device(dev):
+        _capi.check(lib.gh_hair_segments_backward_capturable(
+            sp.n_head, sp.N, sp.W, sp.H, *sp.common(), _ptr(visible), _ptr(geom_buffer),
+            _ptr(g["xyz"]), _ptr(g["dirs"]), _ptr(g["f_dc"]), _ptr(g["f_rest"]), _ptr(g["conf"]), _ptr(nan_flag), 0,
+            _stream(dev)))
+    return g

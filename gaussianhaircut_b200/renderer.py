@@ -26,8 +26,8 @@ import torch.nn.functional as F
 from . import _C, projection
 from ._alloc import empty_rows
 
-__all__ = ["render", "render_hair", "render_hair_strands", "render_hair_strands_capturable", "render_raw",
-           "render_raw_capturable", "set_nan_flag"]
+__all__ = ["render", "render_hair", "render_hair_segments", "render_hair_segments_capturable", "render_hair_strands",
+           "render_hair_strands_capturable", "render_raw", "render_raw_capturable", "set_nan_flag"]
 
 _EMPTY = torch.Tensor([])
 
@@ -74,7 +74,9 @@ class _FusedRender(torch.autograd.Function):
     frozen head block of render_hair().
     Strand models (render_hair_strands, static["strands"] = polyline origins): xyz is None, `dirs` is the (S,L,3) segment
     vector parameter and `scaling` the (1,) strand thickness; the segment midpoints are computed into the means3D rows
-    of this model and kept for the backward, which returns the gradient of `dirs` (S,L,3)."""
+    of this model and kept for the backward, which returns the gradient of `dirs` (S,L,3).
+    Segment models (render_hair_segments: static["cfg"] = HAIR_STRANDS, no static["strands"]): `xyz` (N,3) are the given
+    midpoints and `dirs` (N,3) the segment vectors; both gradients are returned as the projection backward writes them."""
 
     @staticmethod
     def forward(ctx, xyz, scaling, rotation, dirs, f_dc, f_rest, opacity, label, conf, viewspace, viewmatrix, projmatrix,
@@ -292,6 +294,76 @@ def render_hair_strands_capturable(camera: Dict[str, torch.Tensor], pc, pc_hair,
     return _CapturableStrandRender.apply(dirs, pc_hair._features_dc, pc_hair._features_rest, pc_hair._orient_conf, st)
 
 
+class _CapturableSegmentRender(torch.autograd.Function):
+    """The capturable twin of _FusedRender for render_hair_segments: (xyz, dirs, f_dc, f_rest, conf, static) -> (raw
+    image, radii) over the head block and the N segment rows, with the gradients of the five segment tensors.  `static`
+    as in _CapturableStrandRender."""
+
+    @staticmethod
+    def forward(ctx, xyz, dirs, f_dc, f_rest, conf, static):
+        st = static
+        sp = projection.pack_segment_inputs(st["head"], xyz, dirs, st["scale"], f_dc, f_rest, conf, *st["camera"],
+                                            st["W"], st["H"], st["sh_degree"], st["mod"])
+        out, radii, geom, img = projection.hair_segments_forward_binned_capturable(
+            sp, st["binning"], st["capacity"], st["status"], st["num_rendered"])
+        color = _C.forward_render_capturable(st["bg"], out["colors"], geom, st["binning"], img, st["capacity"], sp.H, sp.W)
+        ctx.sp, ctx.st = sp, st
+        ctx.bufs = (out["colors"], out["visible"], radii, geom, img)
+        ctx.mark_non_differentiable(radii)
+        return color, radii
+
+    @staticmethod
+    def backward(ctx, g_color, _g_radii):
+        st = ctx.st
+        colors, visible, radii, geom, img = ctx.bufs
+        _C.backward_records_capturable(st["bg"], colors, radii, geom, st["binning"], img, st["capacity"], g_color)
+        g = projection.hair_segments_backward_capturable(ctx.sp, visible, geom, nan_flag=_NAN_FLAG["t"])
+        need = ctx.needs_input_grad
+        return tuple(g[k] if need[i] else None for i, k in enumerate(("xyz", "dirs", "f_dc", "f_rest", "conf"))) + (None,)
+
+
+def _segment_rows(pc_hair, who: str) -> int:
+    """N, the segment rows of a GaussianModelHair after generate_strands(): `_xyz`, `_dir` (N,3) and N-row features."""
+    xyz, dirs = pc_hair._xyz, pc_hair._dir
+    if xyz.ndim != 2 or xyz.shape[-1] != 3 or tuple(dirs.shape) != tuple(xyz.shape):
+        raise RuntimeError(f"{who}: _xyz and _dir must both be (N, 3), got {tuple(xyz.shape)} and {tuple(dirs.shape)}")
+    N = int(xyz.shape[0])
+    for name in ("_features_dc", "_features_rest", "_orient_conf"):
+        t = getattr(pc_hair, name)
+        if t.shape[0] != N:
+            raise RuntimeError(f"{who}: {name} must have N = {N} rows (strand-major), got {t.shape[0]}")
+    return N
+
+
+def render_hair_segments_capturable(camera: Dict[str, torch.Tensor], pc, pc_hair, bg_color: torch.Tensor, width: int,
+                                    height: int, binning: torch.Tensor, capacity: int, status: torch.Tensor,
+                                    num_rendered: Optional[torch.Tensor] = None, scaling_modifier: float = 1.0):
+    """`render_hair_segments` for CUDA-graph capture (graphs.CapturedLatentStrandStep): the frozen head block of `pc`
+    (None or an empty block: hair only) followed by the N segment rows of `pc_hair`, with no host synchronisation.
+    `camera`, `binning`, `capacity`, `status` and `num_rendered` as in render_hair_strands_capturable.  -> (raw
+    (10,H,W) image, radii (n_head + N,)).  Gradients flow to `_xyz`, `_dir`, `_features_dc`, `_features_rest` and
+    `_orient_conf`; set_nan_flag() works as with render_hair_segments.  With the same inputs, image, radii and
+    (deterministic mode) gradients are bit-identical to render_hair_segments'."""
+    for k in ("viewmatrix", "projmatrix", "campos", "tan_fov"):
+        if camera[k].requires_grad:
+            raise RuntimeError(f"render_hair_segments_capturable: camera tensor '{k}' requires grad; trainable cameras "
+                               "are not supported")
+    projection._check_no_strand_arena()
+    if _segment_rows(pc_hair, "render_hair_segments_capturable") < 1:
+        raise RuntimeError("render_hair_segments_capturable: the model has no segment rows")
+    scale = pc_hair.scale
+    if not isinstance(scale, torch.Tensor):
+        raise RuntimeError("render_hair_segments_capturable: pc_hair.scale must be a (1,) device tensor (a captured "
+                           "launch keeps its address)")
+    head = _head_block(pc) if pc is not None else None
+    st = {"W": int(width), "H": int(height), "bg": bg_color, "mod": float(scaling_modifier),
+          "sh_degree": int(pc_hair.active_sh_degree), "head": head, "scale": scale.detach(),
+          "camera": (camera["viewmatrix"], camera["projmatrix"], camera["campos"], camera["tan_fov"]),
+          "binning": binning, "capacity": int(capacity), "status": status, "num_rendered": num_rendered}
+    return _CapturableSegmentRender.apply(pc_hair._xyz, pc_hair._dir, pc_hair._features_dc, pc_hair._features_rest,
+                                          pc_hair._orient_conf, st)
+
+
 def _post(renders: torch.Tensor, radii: torch.Tensor, viewspace: torch.Tensor) -> Dict[str, torch.Tensor]:
     """The reference's epilogue (gaussian_renderer/__init__.py:98-113)."""
     rendered_image, rendered_mask, rendered_cov2D, rendered_orient_conf, _ = renders.split([3, 2, 3, 1, 1], dim=0)
@@ -424,5 +496,45 @@ def render_hair_strands(viewpoint_camera, pc, pc_hair, pipe, bg_color: torch.Ten
     renders, radii = _FusedRender.apply(
         None, scale.detach(), None, dirs, pc_hair._features_dc, pc_hair._features_rest, None, None, pc_hair._orient_conf,
         viewspace, viewpoint_camera.world_view_transform, viewpoint_camera.full_proj_transform,
+        viewpoint_camera.camera_center, _tanfov_tensor(viewpoint_camera), st)
+    return _post(renders, radii, viewspace)
+
+
+def render_hair_segments(viewpoint_camera, pc, pc_hair, pipe, bg_color: torch.Tensor, scaling_modifier: float = 1.0):
+    """`render_hair` for a GaussianModelHair (src/scene/gaussian_model_latent_strands.py:28) on the fused strand path:
+    same contract and returned dictionary as render_hair, but the strand Gaussians' scales and rotations are derived
+    inside the kernels from the segment vectors, so neither `get_scaling` nor `_rotation` is read.  Read: `_xyz` (N,3)
+    segment midpoints, `_dir` (N,3) segment vectors, `scale` (the strand thickness, a (1,) CUDA tensor or a float),
+    `_features_dc`, `_features_rest`, `_orient_conf` (N rows, strand-major) and `active_sh_degree`.  Autograd carries
+    the gradients of the five tensors back to whatever produced them -- the strand decoder's parameters in training,
+    or leaves -- and also fills `.grad` of `viewspace_points` and of trainable camera tensors; set_nan_flag() works as
+    with render_hair.  `pc` supplies the frozen head block like in render_hair (None or an empty block: hair only).
+
+    A train_latent_strands.py loop replaces `pc_hair.initialize_gaussians_hair(iteration)` -- generate_strands() plus
+    the parallel-transport rotations this function does not need -- with
+
+        diffusion_dict = pc_hair.generate_strands(iteration)
+        pc_hair.LDiff = diffusion_dict.get("L_diff")
+
+    and renders with this function.  The strand model has no gradient-arena layout: an installed arena
+    (projection.set_gradient_arena) raises.
+
+    render_hair_segments_capturable is the CUDA-graph form (graphs.CapturedLatentStrandStep captures render, loss and
+    backward down to the five tensors with it)."""
+    projection._check_no_strand_arena()
+    N = _segment_rows(pc_hair, "render_hair_segments")
+    dev = pc_hair._xyz.device
+    scale = pc_hair.scale
+    if not isinstance(scale, torch.Tensor):
+        scale = torch.full((1,), float(scale), dtype=torch.float32, device=dev)
+    head = _head_block(pc) if pc is not None else None
+    n_head = 0 if head is None else int(head["xyz"].shape[0])
+    viewspace = empty_rows(n_head + N, (3,), torch.float32, dev).requires_grad_(True)
+    st = _static(viewpoint_camera, bg_color, scaling_modifier, pc_hair.active_sh_degree, getattr(pipe, "debug", False),
+                 projection.HAIR_STRANDS)
+    st["head"] = head if n_head > 0 else None
+    renders, radii = _FusedRender.apply(
+        pc_hair._xyz, scale.detach(), None, pc_hair._dir, pc_hair._features_dc, pc_hair._features_rest, None, None,
+        pc_hair._orient_conf, viewspace, viewpoint_camera.world_view_transform, viewpoint_camera.full_proj_transform,
         viewpoint_camera.camera_center, _tanfov_tensor(viewpoint_camera), st)
     return _post(renders, radii, viewspace)

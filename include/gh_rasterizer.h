@@ -497,6 +497,48 @@ int gh_hair_strands_backward_capturable(
     unsigned int* nan_flag, int debug, gh_stream_t stream);
 
 /*
+ * Capturable latent strand iteration (DESIGN §20): render_hair_segments -- the frozen head block of n_head Gaussians
+ * followed by N given segment rows -- under the contract of the gh_hair_strands_*_capturable pair above.  The only
+ * difference: the segment rows come as their midpoints `xyz` (N,3) and segment vectors `dirs` (N,3), the layout
+ * GaussianModelHair.generate_strands leaves in _xyz and _dir (N = num_strands * (strand_length - 1), strand-major),
+ * instead of as polylines.  So the forward runs no gh_strand_midpoints (xyz is read in place) and the backward no
+ * gh_strand_backward (no cumulative sum to chain through).
+ *
+ * gh_hair_segments_forward_binned_capturable: the head rows projected with `head_flags` (no strand bit) and
+ *   `head_det_eps`, the segment rows with `flags` (strand bit set; `scale` = one device float, the strand thickness)
+ *   and `det_eps`, then one tile histogram, scan, capacity guard and emit over all P = n_head + N rows.  Outputs,
+ *   status and num_rendered as in gh_hair_strands_forward_binned_capturable.  n_head >= 0, N >= 0, 3 * N and
+ *   n_head + N below 2^31, P > 0; xyz and dirs are required even when N == 0.
+ * gh_hair_segments_backward_capturable: after gh_backward_capturable, the strand-mode projection backward reads the
+ *   accumulation records of rows [n_head, P) in place from `geom_buffer` and writes dL/dxyz to d_xyz (N,3), dL/ddirs to
+ *   d_dirs (N,3), and d_features_dc, d_features_rest, d_orient_conf (may be NULL).  nan_flag (device uint32, may be
+ *   NULL) as in gh_project_backward.  No head-row and no camera gradients.  N > 0.
+ */
+int gh_hair_segments_forward_binned_capturable(
+    int n_head, int N, int width, int height,
+    const float* head_xyz, const float* head_scaling, const float* head_rotation,
+    const float* head_features_dc, const float* head_features_rest, const float* head_opacity,
+    unsigned int head_flags, float head_det_eps,
+    const float* xyz, const float* dirs, const float* scale,
+    const float* features_dc, const float* features_rest, const float* orient_conf,
+    unsigned int flags, float det_eps,
+    const float* viewmatrix, const float* projmatrix, const float* campos,
+    const float* tan_fov, float scale_modifier, int sh_degree,
+    float* means2D, float* colors, float* opacities, float* conic, unsigned char* visible,
+    int* radii, char* geom_buffer, char* img_buffer, char* binning_buffer, long long capacity,
+    unsigned int* status, unsigned int* num_rendered, int debug, gh_stream_t stream);
+int gh_hair_segments_backward_capturable(
+    int n_head, int N, int width, int height,
+    const float* xyz, const float* dirs, const float* scale,
+    const float* features_dc, const float* features_rest, const float* orient_conf,
+    unsigned int flags, float det_eps,
+    const float* viewmatrix, const float* projmatrix, const float* campos,
+    const float* tan_fov, float scale_modifier, int sh_degree,
+    const unsigned char* visible, const char* geom_buffer,
+    float* d_xyz, float* d_dirs, float* d_features_dc, float* d_features_rest, float* d_orient_conf,
+    unsigned int* nan_flag, int debug, gh_stream_t stream);
+
+/*
  * Trainable cameras (DESIGN §17): the reference's BARF camera model (src/scene/cameras.py:95-152, use_barf = True) and
  * its camera Adam (src/train_gaussians.py:45-63, 183-196).  A rig of n cameras owns, on the device:
  *   base       float[n][18]  C = the float32 _colmap_transform (16, row-major), FoVx, FoVy (the camera's base state)

@@ -88,6 +88,9 @@ SIGNATURES = {
     "gh_allreduce_p2p": (_i, [_p, _p, C.c_ulonglong, _i, _i, C.c_size_t, C.c_size_t, C.c_uint, _p, _p, _p]),
     "gh_image_loss": (_i, [_i, _i, _p, _p, _p, _p, _p, _f, _f, _f, _f, _p, _p, _p, _p, _i]),
     "gh_image_loss_stage": (_i, [_i, _i, _i, C.c_uint, _p, _p, _p, _p, _p, _f, _f, _f, _f, _p, _p, _p, _p, _i]),
+    "gh_render_maps": (_i, [_i, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),   # W H out_color angle conf_masked render hair head orient orient_vis conf_vis stream
+    "gh_eval_metrics_workspace_size": (_i, [_i, _i, C.POINTER(_sz)]),
+    "gh_eval_metrics": (_i, [_i, _i, _i, _p, _p, _p, _p, _p, _p, _sz, _p, _p]),   # W H stage out_color gt_image gt_mask gt_angle gt_conf workspace bytes row stream
     "gh_project_workspace_size": (_i, [_i, C.POINTER(C.c_size_t)]),
     "gh_project_forward": (_i, _PROJ_ARGS + [
         _p, _p, _p, _p, _p, _p,              # means2D colors opacities conic cov3D visible

@@ -22,6 +22,7 @@
 // orientation confidence 8, depth 9.
 #include "gh_common.cuh"
 #include "gh_kernels.h"
+#include "gh_image_math.cuh"
 #include "../../include/gh_rasterizer.h"
 
 namespace {
@@ -66,61 +67,9 @@ __device__ __forceinline__ void gh_block_add(double v, double* dst, double* s_pa
 // completion tickets of the three summing kernels (uint32, zeroed with the sums)
 enum { GH_TK_PRESUM = 8, GH_TK_POINTWISE = 9, GH_TK_MAIN = 10 };
 
-// Deterministic variant of gh_block_add for K sums (gh_image_loss with deterministic != 0): warp shuffle tree, the 8
-// warps in warp order, then the CTA's total goes to its own slot part[k * gridDim + CTA] -- no floating-point atomics.
-// The last CTA to finish (ticket) adds the slots in CTA order into sums[idx[k]], staging 256 slots at a time in shared
-// memory; that is one of the orders the per-CTA atomicAdd could produce, now the only one, so the loss values and the
-// 1 / sum(w) that scales the orientation gradient are reproducible.
-template <int K>
-__device__ __forceinline__ void gh_block_sum_fixed(double (&v)[K], double* __restrict__ part, double* sums,
-                                                   const int (&idx)[K], int ticket_slot) {
-    __shared__ double s_part[K][8];
-    __shared__ bool s_last;
-    const int tid = threadIdx.x;
-#pragma unroll
-    for (int k = 0; k < K; k++) {
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], o);
-    }
-    __syncthreads();
-    if ((tid & 31) == 0) {
-#pragma unroll
-        for (int k = 0; k < K; k++) s_part[k][tid >> 5] = v[k];
-    }
-    __syncthreads();
-    const unsigned G = gridDim.x * gridDim.y, b = blockIdx.y * gridDim.x + blockIdx.x;
-    if (tid == 0) {
-#pragma unroll
-        for (int k = 0; k < K; k++) {
-            double t = 0.0;
-            for (int w = 0; w < 8; w++) t += s_part[k][w];
-            part[(size_t)k * G + b] = t;
-        }
-        __threadfence();
-        s_last = atomicAdd(reinterpret_cast<unsigned*>(sums + ticket_slot), 1u) == G - 1u;
-    }
-    __syncthreads();
-    if (!s_last) return;
-    __threadfence();
-    __shared__ double s_stage[K][256];
-    double t = 0.0;                     // thread k: sum k
-    for (unsigned c0 = 0; c0 < G; c0 += 256) {
-        const unsigned m = min(256u, G - c0);
-#pragma unroll
-        for (int k = 0; k < K; k++)
-            if ((unsigned)tid < m) s_stage[k][tid] = __ldcg(part + (size_t)k * G + c0 + tid);
-        __syncthreads();
-        if (tid < K)
-            for (unsigned i = 0; i < m; i++) t += s_stage[tid][i];
-        __syncthreads();
-    }
-    if (tid < K) {
-        int d = idx[0];
-#pragma unroll
-        for (int k = 1; k < K; k++) d = (tid == k) ? idx[k] : d;
-        sums[d] = t;
-    }
-}
+// The deterministic variant (gh_image_loss with deterministic != 0) is gh_block_sum_fixed (gh_image_math.cuh): per-CTA
+// slots added in CTA order by the last CTA, so the loss values and the 1 / sum(w) that scales the orientation gradient
+// are reproducible.
 
 // per-CTA slots of the three summing kernels, after the sums: presum, pointwise (3 sums), SSIM
 struct GhLossParts {
@@ -186,15 +135,10 @@ __device__ __forceinline__ void gh_loss_pointwise(const GhLossParams& prm, size_
     if constexpr (STAGE == 2) dL[4 * plane + pi] = 0.f;
     // orientation: dir = normalize(out[5:7]), mirrored so that dir.x >= 0, angle = acos(dir.y)/pi
     const float c5 = out[5 * plane + pi], c6 = out[6 * plane + pi], conf = no_conf ? 1.f : out[8 * plane + pi];
-    const float nrm = sqrtf(c5 * c5 + c6 * c6);
-    const float den = fmaxf(nrm, 1e-12f);                  // F.normalize eps
-    const float dirx = c5 / den, diry = c6 / den;
-    const float mirror = (dirx < 0.f) ? -1.f : 1.f;
-    const float lo = -1.f + 1e-3f, hi = 1.f - 1e-3f;
-    const float tcl = fminf(fmaxf(diry, lo), hi);
-    const float t = tcl * mirror;
-    const float PI = 3.14159265358979323846f;
-    const float ang = acosf(t) / PI;
+    const GhOrientAngle oa = gh_orient_angle(c5, c6);
+    const float nrm = oa.nrm, diry = oa.diry, mirror = oa.mirror, t = oa.t, ang = oa.ang;
+    const float lo = GH_ORIENT_LO, hi = GH_ORIENT_HI;
+    const float PI = GH_PI_F;
     const float g = gt_angle[pi];
     const float d0 = ang - g, d1 = d0 - 1.f, d2 = d0 + 1.f;
     const float l0 = fabsf(d0), l1 = fabsf(d1), l2 = fabsf(d2);

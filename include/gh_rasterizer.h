@@ -276,6 +276,49 @@ int gh_image_loss_stage(int width, int height, int stage, unsigned options,
                         void* workspace, float* losses, float* dL_dout, gh_stream_t stream, int deterministic);
 
 /*
+ * Rendering without a backward: the maps src/render_gaussians.py:50-68 and src/render_strands.py:51-69 write for every
+ * view, from the raw out_color (10,H,W) in one pass.  Every output is optional (NULL: not wanted):
+ *   orient_angle        float (H,W)    the epilogue of src/gaussian_renderer/__init__.py:100-105, the same device code
+ *                                      as the image losses
+ *   orient_conf_masked  float (H,W)    orient_conf * hair_mask (what the scripts torch.save to orient_confs/)
+ *   render_u8           uint8 (H,W,3)  save_image(render), interleaved RGB
+ *   hair_mask_u8, head_mask_u8  uint8 (H,W)   save_image(mask[:1]), save_image(mask[1:])
+ *   orient_u8           uint8 (H,W)    save_image(orient_angle * hair_mask)
+ *   orient_vis_u8       uint8 (H,W,3)  save_image(vis_orient(orient_angle, hair_mask))  (src/utils/image_utils.py:22-37)
+ *   orient_conf_vis_u8  uint8 (H,W,3)  save_image(vis_orient(orient_angle, 1 - 1 / (orient_conf * hair_mask + 1)))
+ * save_image's bytes are x.mul(255).add_(0.5).clamp_(0, 255).to(uint8); every float operation here is rounded on its
+ * own like the tensor code (no FMA contraction), so the bytes are those of that composition on the same raw image.
+ * A NaN value becomes byte 0.  The byte maps must be 4-byte aligned.  One launch on `stream`, no allocation, no host
+ * synchronisation; refuses (GH_E_INVALID_ARG, before any launch) bad sizes, a NULL out_color, more than 2^27 pixels.
+ */
+int gh_render_maps(int width, int height, const float* out_color, float* orient_angle, float* orient_conf_masked,
+                   unsigned char* render_u8, unsigned char* hair_mask_u8, unsigned char* head_mask_u8,
+                   unsigned char* orient_u8, unsigned char* orient_vis_u8, unsigned char* orient_conf_vis_u8,
+                   gh_stream_t stream);
+
+/*
+ * One view's numbers of the trainers' training_report, from the raw out_color and the view's ground truth maps (as
+ * gh_image_loss takes them), written to row (device float[8]) -- a caller evaluating N views hands in row i of an
+ * (N,8) buffer and reads it back once.  stage: GH_LOSS_STAGE_*.
+ *   APPEARANCE, STRANDS (src/train_gaussians.py:254-277, src/train_strands.py): render, mask, orient_angle and their
+ *     ground truths clamped to [0,1]; l1 = mean |image - gt|; mask = mean |mask - gt_mask| over both channels;
+ *     or = or_loss(angle, gt_angle, mask=gt_mask[:1], weight=gt_orient_conf); psnr = mean over the three channels of
+ *     20 log10(1 / sqrt(mse_c)).
+ *   LATENT_STRANDS (src/train_latent_strands.py:235-258): image and gt multiplied by gt_mask[:1] before l1 and psnr;
+ *     ce_loss(mask[:1], gt_mask[:1]) in place of the mask term.
+ * row: l1, mask or ce, or, psnr, ssim, mse_r, mse_g, mse_b.  The ssim slot is NaN: it is not computed.  A zero weight
+ *   sum gives or = NaN (0 / 0) and mse_c = 0 gives psnr = inf, like the reference.
+ * The sums are formed in a fixed order (per-CTA slots in the workspace, added in CTA order by the last CTA, in double):
+ * the row is bit-identical run to run.  workspace: gh_eval_metrics_workspace_size bytes, 8-byte aligned.  Three stream
+ * operations (memset + 2 launches), no allocation, no host synchronisation; refuses (GH_E_INVALID_ARG, before any CUDA
+ * call) bad sizes, a NULL pointer, an unknown stage, a workspace that is misaligned or smaller than the size query's.
+ */
+int gh_eval_metrics_workspace_size(int width, int height, size_t* bytes);
+int gh_eval_metrics(int width, int height, int stage, const float* out_color, const float* gt_image,
+                    const float* gt_mask, const float* gt_orient_angle, const float* gt_orient_conf,
+                    void* workspace, size_t workspace_bytes, float* row, gh_stream_t stream);
+
+/*
  * Multi-GPU (SURVEY.md 8e): sum a float32 buffer that lives in SYMMETRIC memory (the same allocation on
  * every GPU of the node, each mapped into every process, e.g. torch.distributed._symmetric_memory) over
  * all ranks, in place, with one kernel per rank that reads and writes its peers' copies through NVLink.

@@ -22,11 +22,12 @@ GH_E_NO_COLORS = 2
 GH_E_CUDA = 3
 GH_E_PREFILTERED = 4
 
-ABI_VERSION = 5
+ABI_VERSION = 6
 
 _p = C.c_void_p
 _i = C.c_int
 _f = C.c_float
+_d = C.c_double
 _ll = C.c_longlong
 _sz = C.c_size_t
 
@@ -83,7 +84,7 @@ SIGNATURES = {
         _i, _p,                              # debug stream
         _p, _sz]),                           # det_buffer det_bytes (NULL, 0: the fast path)
     "gh_mark_visible": (_i, [_i, _p, _p, _p, _p, _p]),
-    "gh_adam_step": (_i, [_i, _p, _p, _p, _p, _p, _p, _f, _f, _f, _i, _p, _p, _p, _p]),
+    "gh_adam_step": (_i, [_i, _p, _p, _p, _p, _p, _p, _d, _d, _f, _i, _p, _p, _p, _p]),
     "gh_image_loss_workspace_size": (_i, [_i, _i, C.POINTER(C.c_size_t)]),
     "gh_allreduce_p2p": (_i, [_p, _p, C.c_ulonglong, _i, _i, C.c_size_t, C.c_size_t, C.c_uint, _p, _p, _p]),
     "gh_image_loss": (_i, [_i, _i, _p, _p, _p, _p, _p, _f, _f, _f, _f, _p, _p, _p, _p, _i]),
@@ -119,7 +120,7 @@ SIGNATURES = {
         _p, _p, _p, _p, _p, _p,              # d_xyz d_scaling d_rotation d_dirs d_features_dc d_features_rest
         _p, _p, _p, _p, _p,                  # d_opacity d_label d_orient_conf d_means2D d_camera
         _p, _p, _i, _p]),                    # nan_flag workspace debug stream
-    "gh_adam_step_capturable": (_i, [_i, _p, _p, _p, _p, _p, _p, _f, _f, _f, _p, _p, _p, _i, _p]),
+    "gh_adam_step_capturable": (_i, [_i, _p, _p, _p, _p, _p, _p, _d, _d, _f, _p, _p, _p, _i, _p]),
     "gh_hair_strands_forward_binned_capturable": (_i, [
         _i, _i, _i, _i, _i,                  # n_head S L width height
         _p, _p, _p, _p, _p, _p,              # head: xyz scaling rotation features_dc features_rest opacity
@@ -170,7 +171,7 @@ SIGNATURES = {
     "gh_orient_gabor": (_i, [_i, _i, _p, _i, _i, _i, _p, _p, _p, _p, _sz, _p]),  # H W bank N K nf thetas orients var ws bytes stream
     "gh_camera_forward": (_i, [_i, _p, _p, _p, _p, _p, _p, _p, _p, _i, _p]),   # n residuals base index view proj campos tan status debug stream
     "gh_camera_backward": (_i, [_i, _p, _p, _p, _i, _p, _p, _p, _p, _p, _i, _p]),   # n residuals base index intrinsics d_camera grad touched nan status debug stream
-    "gh_camera_adam_step": (_i, [_i, _i, _p, _p, _p, _p, _p, _p, _p, _f, _f, _f, _p, _p, _i, _p]),   # n intrinsics r grad touched m v steps lrs b1 b2 eps nan skip debug stream
+    "gh_camera_adam_step": (_i, [_i, _i, _p, _p, _p, _p, _p, _p, _p, _d, _d, _f, _p, _p, _i, _p]),   # n intrinsics r grad touched m v steps lrs b1 b2 eps nan skip debug stream
 }
 
 _lib = None

@@ -45,28 +45,37 @@ gh_adam_nan_kernel(GhAdamGroups g, unsigned int* __restrict__ flag)
     if (__any_sync(0xffffffffu, bad) && (threadIdx.x & 31) == 0) atomicOr(flag, 1u);
 }
 
-// DEV_LR: the learning rates are read from device memory (lr_dev[group]) instead of the launch argument
+// DEV_LR: the learning rates are read from device memory (lr_dev[group]) instead of the launch argument.
+// `step` (1-based) is used when step_state is NULL.
 template <bool DEV_LR>
 __device__ __forceinline__ void
-gh_adam_update_body(const GhAdamGroups& g, const float* __restrict__ lr_dev, float beta1, float beta2, float eps,
-                    float bc1, float bc2_sqrt, const unsigned int* __restrict__ flag,
+gh_adam_update_body(const GhAdamGroups& g, const float* __restrict__ lr_dev, double beta1, double beta2, float eps,
+                    int step, const unsigned int* __restrict__ flag,
                     const unsigned int* __restrict__ skip_flag, int* step_state)
 {
-    if (flag != nullptr && *flag != 0u) return;     // a gradient held a NaN: skip this step entirely
-    if (skip_flag != nullptr && *skip_flag != 0u) return;   // the producer of the gradients reported a failure
-    if (step_state != nullptr) {
-        // device-resident step count (only advanced by steps that were not skipped, like torch's state['step'])
-        const int step = step_state[0] + 1;
-        bc1 = gh_adam_bc1(beta1, step);
-        bc2_sqrt = gh_adam_bc2_sqrt(beta2, step);
-    }
+    // thread 0 reads the flags and the step count and derives the constants once per CTA; nothing else reads them
+    __shared__ GhAdamConst c_sh;
+    __shared__ int skip_sh;
     const int k = blockIdx.y;
+    if (threadIdx.x == 0) {
+        // independent loads, issued together
+        const unsigned int nan_seen = flag != nullptr ? *flag : 0u, skip_seen = skip_flag != nullptr ? *skip_flag : 0u;
+        const int taken = step_state != nullptr ? step_state[0] : 0;
+        const float lr = DEV_LR ? lr_dev[k] : g.lr[k];
+        // a gradient held a NaN, or the producer of the gradients reported a failure: skip this step entirely
+        skip_sh = (nan_seen | skip_seen) != 0u;
+        // device-resident step count (only advanced by steps that were not skipped, like torch's state['step'])
+        if (step_state != nullptr) step = taken + 1;
+        if (!skip_sh) c_sh = gh_adam_const(beta1, beta2, eps, lr, gh_adam_bias(beta1, beta2, step));
+    }
+    __syncthreads();
+    if (skip_sh) return;
+    const GhAdamConst c = c_sh;
     const unsigned long long n = g.end[k] - (k ? g.end[k - 1] : 0ull);
     float* __restrict__ P = g.param[k];
     const float* __restrict__ G = g.grad[k];
     float* __restrict__ M = g.exp_avg[k];
     float* __restrict__ V = g.exp_avg_sq[k];
-    const GhAdamConst c = gh_adam_const(beta1, beta2, eps, DEV_LR ? lr_dev[k] : g.lr[k], bc1, bc2_sqrt);
     const unsigned long long tid = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
     const unsigned long long nthreads = (unsigned long long)gridDim.x * blockDim.x;
     unsigned long long done = 0;
@@ -90,8 +99,10 @@ gh_adam_update_body(const GhAdamGroups& g, const float* __restrict__ lr_dev, flo
         P[i] = p; M[i] = m; V[i] = v;
     }
     if (step_state != nullptr) {
-        // the last CTA to finish advances the counter (every CTA has read it by then)
+        // the last CTA to finish advances the counter: every CTA's thread 0 read it before the __syncthreads() above,
+        // and this one waits for the whole CTA before it counts itself done
         __threadfence();
+        __syncthreads();
         if (threadIdx.x == 0) {
             const unsigned int t = atomicAdd(reinterpret_cast<unsigned int*>(step_state + 1), 1u);
             if (t == gridDim.x * gridDim.y - 1) { step_state[0] += 1; step_state[1] = 0; }
@@ -100,20 +111,19 @@ gh_adam_update_body(const GhAdamGroups& g, const float* __restrict__ lr_dev, flo
 }
 
 __global__ void __launch_bounds__(256)
-gh_adam_update_kernel(GhAdamGroups g, float beta1, float beta2, float eps,
-                      float bc1, float bc2_sqrt, const unsigned int* __restrict__ flag,
-                      const unsigned int* __restrict__ skip_flag, int* step_state)
+gh_adam_update_kernel(GhAdamGroups g, double beta1, double beta2, float eps, int step,
+                      const unsigned int* __restrict__ flag, const unsigned int* __restrict__ skip_flag, int* step_state)
 {
-    gh_adam_update_body<false>(g, nullptr, beta1, beta2, eps, bc1, bc2_sqrt, flag, skip_flag, step_state);
+    gh_adam_update_body<false>(g, nullptr, beta1, beta2, eps, step, flag, skip_flag, step_state);
 }
 
 // gh_adam_step_capturable: learning rates from device memory, step count always on the device
 __global__ void __launch_bounds__(256)
-gh_adam_update_dev_lr_kernel(GhAdamGroups g, const float* __restrict__ lrs, float beta1, float beta2, float eps,
+gh_adam_update_dev_lr_kernel(GhAdamGroups g, const float* __restrict__ lrs, double beta1, double beta2, float eps,
                              const unsigned int* __restrict__ flag, const unsigned int* __restrict__ skip_flag,
                              int* step_state)
 {
-    gh_adam_update_body<true>(g, lrs, beta1, beta2, eps, 0.f, 0.f, flag, skip_flag, step_state);
+    gh_adam_update_body<true>(g, lrs, beta1, beta2, eps, 0, flag, skip_flag, step_state);
 }
 
 }  // namespace
@@ -148,7 +158,7 @@ static int gh_adam_groups(const char* who, int n_groups, float* const* params, c
 extern "C" int gh_adam_step(int n_groups, float* const* params, const float* const* grads,
                             float* const* exp_avg, float* const* exp_avg_sq,
                             const unsigned long long* sizes, const float* lrs,
-                            float beta1, float beta2, float eps, int step, int* step_state,
+                            double beta1, double beta2, float eps, int step, int* step_state,
                             unsigned int* nan_flag, const unsigned int* skip_flag, gh_stream_t stream_)
 {
     cudaStream_t stream = (cudaStream_t)stream_;
@@ -160,21 +170,19 @@ extern "C" int gh_adam_step(int n_groups, float* const* params, const float* con
     dim3 grid;
     const int rc = gh_adam_groups("gh_adam_step", n_groups, params, grads, exp_avg, exp_avg_sq, sizes, lrs, g, total, grid);
     if (rc != GH_OK || total == 0) return rc;
-    const double bc1 = 1.0 - pow((double)beta1, (double)(step < 1 ? 1 : step));
-    const double bc2 = 1.0 - pow((double)beta2, (double)(step < 1 ? 1 : step));
     if (nan_flag) {
         const cudaError_t e = cudaMemsetAsync(nan_flag, 0, sizeof(unsigned int), stream);
         if (e != cudaSuccess) return gh_cuda_status("gh_adam_step", "memset(NaN flag)", e);
         gh_adam_nan_kernel<<<grid, 256, 0, stream>>>(g, nan_flag);
     }
-    gh_adam_update_kernel<<<grid, 256, 0, stream>>>(g, beta1, beta2, eps, (float)bc1, (float)sqrt(bc2), nan_flag, skip_flag, step_state);
+    gh_adam_update_kernel<<<grid, 256, 0, stream>>>(g, beta1, beta2, eps, step, nan_flag, skip_flag, step_state);
     return gh_launch_status("gh_adam_step", nan_flag ? 2 : 1);
 }
 
 extern "C" int gh_adam_step_capturable(int n_groups, float* const* params, const float* const* grads,
                                        float* const* exp_avg, float* const* exp_avg_sq,
                                        const unsigned long long* sizes, const float* lrs,
-                                       float beta1, float beta2, float eps, int* step_state,
+                                       double beta1, double beta2, float eps, int* step_state,
                                        unsigned int* nan_flag, const unsigned int* skip_flag, int debug, gh_stream_t stream_)
 {
     const char* who = "gh_adam_step_capturable";

@@ -216,7 +216,7 @@ int gh_forward_phase1_capturable(const char* who, int P, int width, int height, 
 
 extern "C" {
 
-int gh_abi_version(void) { return 5; }
+int gh_abi_version(void) { return 6; }
 
 unsigned long long gh_kernel_launch_count(void) { return g_launches.load(); }
 

@@ -67,7 +67,7 @@ gh_camera_backward_kernel(int n, const float* __restrict__ residuals, const floa
 __global__ void __launch_bounds__(256)
 gh_camera_adam_kernel(int n, int cols, float* __restrict__ residuals, float* __restrict__ grad, int* __restrict__ touched,
                       float* __restrict__ exp_avg, float* __restrict__ exp_avg_sq, int* __restrict__ steps,
-                      const float* __restrict__ lrs, float beta1, float beta2, float eps, unsigned int* nan_flag,
+                      const float* __restrict__ lrs, double beta1, double beta2, float eps, unsigned int* nan_flag,
                       const unsigned int* skip_flag)
 {
     const bool skip = (nan_flag != nullptr && *nan_flag != 0u) || (skip_flag != nullptr && *skip_flag != 0u);
@@ -77,9 +77,9 @@ gh_camera_adam_kernel(int n, int cols, float* __restrict__ residuals, float* __r
         const size_t o = (size_t)i * GH_CAM_ROW;
         if (!skip) {
             const int step = steps[i] + 1;
-            const float bc1 = gh_adam_bc1(beta1, step), bc2_sqrt = gh_adam_bc2_sqrt(beta2, step);
+            const GhAdamBias b = gh_adam_bias(beta1, beta2, step);
             for (int k = 0; k < cols; k++) {
-                const GhAdamConst c = gh_adam_const(beta1, beta2, eps, lr[k < 3 ? 0 : (k < 6 ? 1 : 2)], bc1, bc2_sqrt);
+                const GhAdamConst c = gh_adam_const(beta1, beta2, eps, lr[k < 3 ? 0 : (k < 6 ? 1 : 2)], b);
                 float p = residuals[o + k], m = exp_avg[o + k], v = exp_avg_sq[o + k];
                 gh_adam_elem(p, grad[o + k], m, v, c);
                 residuals[o + k] = p; exp_avg[o + k] = m; exp_avg_sq[o + k] = v;
@@ -139,7 +139,7 @@ extern "C" int gh_camera_backward(int n, const float* residuals, const float* ba
 
 extern "C" int gh_camera_adam_step(int n, int intrinsics, float* residuals, float* grad, int* touched,
                                    float* exp_avg, float* exp_avg_sq, int* steps, const float* lrs,
-                                   float beta1, float beta2, float eps, unsigned int* nan_flag,
+                                   double beta1, double beta2, float eps, unsigned int* nan_flag,
                                    const unsigned int* skip_flag, int debug, gh_stream_t stream_)
 {
     const char* who = "gh_camera_adam_step";

@@ -213,7 +213,7 @@ int gh_debug_export(
 int gh_adam_step(int n_groups, float* const* params, const float* const* grads,
                  float* const* exp_avg, float* const* exp_avg_sq,
                  const unsigned long long* sizes, const float* lrs,
-                 float beta1, float beta2, float eps, int step, int* step_state,
+                 double beta1, double beta2, float eps, int step, int* step_state,
                  unsigned int* nan_flag, const unsigned int* skip_flag, gh_stream_t stream);
 
 /*
@@ -488,7 +488,7 @@ int gh_project_backward_capturable(
 int gh_adam_step_capturable(int n_groups, float* const* params, const float* const* grads,
                             float* const* exp_avg, float* const* exp_avg_sq,
                             const unsigned long long* sizes, const float* lrs,
-                            float beta1, float beta2, float eps, int* step_state,
+                            double beta1, double beta2, float eps, int* step_state,
                             unsigned int* nan_flag, const unsigned int* skip_flag, int debug, gh_stream_t stream);
 
 /*
@@ -621,7 +621,7 @@ int gh_camera_backward(int n, const float* residuals, const float* base, const i
                        unsigned int* status, int debug, gh_stream_t stream);
 int gh_camera_adam_step(int n, int intrinsics, float* residuals, float* grad, int* touched,
                         float* exp_avg, float* exp_avg_sq, int* steps, const float* lrs,
-                        float beta1, float beta2, float eps, unsigned int* nan_flag,
+                        double beta1, double beta2, float eps, unsigned int* nan_flag,
                         const unsigned int* skip_flag, int debug, gh_stream_t stream);
 
 /*

@@ -43,6 +43,27 @@ def parallel_transport(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
     return torch.cat([s, v], dim=-1)
 
 
+# torch's CPU elementwise kernels split a tensor of more than 32768 elements into one part per thread, and whether an
+# element falls in a part's vectorised loop or in its scalar remainder -- which round sigmoid / exp differently --
+# depends on where the parts start, so the float32 bits of a large scene would depend on the machine's thread count.  The
+# scenes apply them part by part as torch does with 16 threads (the split the stored reference records were made with),
+# each part on one thread: the same bits on every machine.
+_GRAIN, _THREADS = 32768, 16
+
+
+def _fixed_chunks(fn, x: torch.Tensor) -> torch.Tensor:
+    flat = x.reshape(-1)
+    n = flat.numel()
+    size = -(-n // max(1, min(_THREADS, -(-n // _GRAIN))))
+    prev = torch.get_num_threads()
+    torch.set_num_threads(1)
+    try:
+        out = torch.cat([fn(flat[i:i + size]) for i in range(0, n, size)])
+    finally:
+        torch.set_num_threads(prev)
+    return out.reshape(x.shape)
+
+
 def make_strand_scene(num_strands: int, seed: int = 0, opacity_mode: str = "random",
                       segments: int = 100) -> Dict[str, torch.Tensor]:
     """CPU float32 tensors of the strands(S) scene: P = segments * num_strands Gaussians."""
@@ -65,7 +86,7 @@ def make_strand_scene(num_strands: int, seed: int = 0, opacity_mode: str = "rand
     scaling = torch.full((P, 3), 2e-4)
     scaling[:, 0] = dirv.norm(dim=-1) * 0.5
     if opacity_mode == "random":
-        opacity = torch.sigmoid(1 + torch.randn(P, 1, generator=g))
+        opacity = _fixed_chunks(torch.sigmoid, 1 + torch.randn(P, 1, generator=g))
     elif opacity_mode == "ones":                                        # real hair: opacity == 1
         _ = torch.randn(P, 1, generator=g)
         opacity = torch.ones(P, 1)
@@ -73,8 +94,8 @@ def make_strand_scene(num_strands: int, seed: int = 0, opacity_mode: str = "rand
         raise ValueError(opacity_mode)
     f_dc = (torch.rand(P, 1, 3, generator=g) - 0.5) / SH_C0
     f_rest = 0.1 * torch.randn(P, 15, 3, generator=g)
-    label = torch.sigmoid(torch.randn(P, 1, generator=g))
-    orient_conf = torch.exp(0.1 * torch.randn(P, 1, generator=g))
+    label = _fixed_chunks(torch.sigmoid, torch.randn(P, 1, generator=g))
+    orient_conf = _fixed_chunks(torch.exp, 0.1 * torch.randn(P, 1, generator=g))
     return {"xyz": xyz.contiguous(), "dir": dirv.contiguous(), "rotation": rotation.contiguous(),
             "scaling": scaling.contiguous(), "opacity": opacity.contiguous(),
             "f_dc": f_dc.contiguous(), "f_rest": f_rest.contiguous(),
@@ -88,11 +109,11 @@ def make_blob_scene(P: int, seed: int = 0, spread: float = 0.25, max_scale: floa
     xyz = spread * torch.randn(P, 3, generator=g)
     scaling = max_scale * torch.rand(P, 3, generator=g) + 1e-4
     rotation = F.normalize(torch.randn(P, 4, generator=g), dim=-1) * (0.5 + torch.rand(P, 1, generator=g))
-    opacity = torch.sigmoid(torch.randn(P, 1, generator=g))
+    opacity = _fixed_chunks(torch.sigmoid, torch.randn(P, 1, generator=g))
     f_dc = (torch.rand(P, 1, 3, generator=g) - 0.5) / SH_C0
     f_rest = 0.1 * torch.randn(P, 15, 3, generator=g)
-    label = torch.sigmoid(torch.randn(P, 1, generator=g))
-    orient_conf = torch.exp(0.1 * torch.randn(P, 1, generator=g))
+    label = _fixed_chunks(torch.sigmoid, torch.randn(P, 1, generator=g))
+    orient_conf = _fixed_chunks(torch.exp, 0.1 * torch.randn(P, 1, generator=g))
     dirv = F.normalize(torch.randn(P, 3, generator=g), dim=-1) * scaling.max(dim=-1, keepdim=True).values
     return {"xyz": xyz, "dir": dirv, "rotation": rotation.contiguous(), "scaling": scaling, "opacity": opacity,
             "f_dc": f_dc, "f_rest": f_rest, "label": label, "orient_conf": orient_conf}

@@ -27,8 +27,9 @@ def _header_params(name):
 
 def test_abi_surface(lib):
     from gaussianhaircut_b200 import _capi
-    # ABI 5: one entry point per forward phase; the optional binning buffer is part of each signature
-    assert lib.gh_abi_version() == _capi.ABI_VERSION == 5
+    # one entry point per forward phase since ABI 5 (the optional binning buffer is part of each signature); ABI 6 takes
+    # the Adam betas as double
+    assert lib.gh_abi_version() == _capi.ABI_VERSION == 6
     sig = _capi.SIGNATURES
     for name in ("gh_forward_preprocess_ex", "gh_forward_render_ex", "gh_project_forward_binned_ex"):
         assert name not in sig and not hasattr(lib, name), name

@@ -24,7 +24,7 @@ def _det_bytes(lib, P, R):
 
 def test_abi_surface(lib):
     from gaussianhaircut_b200 import _capi
-    assert _capi.ABI_VERSION == 5 and lib.gh_abi_version() == 5
+    assert _capi.ABI_VERSION == 6 and lib.gh_abi_version() == 6
     res, args = _capi.SIGNATURES["gh_backward_det_workspace_size"]
     assert res is C.c_int and args == [C.c_int, C.c_longlong, C.POINTER(C.c_size_t)]
     args = _capi.SIGNATURES["gh_backward"][1]

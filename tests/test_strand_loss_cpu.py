@@ -2,7 +2,7 @@
 reference's own loss functions composed as the strand trainers compose them (tests/golden/loss64strands.npz,
 tests/golden/make_golden_loss64_strands.py) and on float64 autograd of the restated compositions; check that stage 0
 is the appearance replay; check that gh_image_loss_stage refuses bad stages, options and arguments before launching
-anything, and that it is declared, exported and bound at ABI 5."""
+anything, and that it is declared, exported and bound at ABI 6."""
 import ctypes as C
 import os
 import re
@@ -195,7 +195,7 @@ def test_appearance_messages_unchanged(lib):
     assert lib.gh_last_error() == b"gh_image_loss: bad size or missing pointer"
 
 
-def test_stage_entry_point_declared_exported_abi5(lib):
+def test_stage_entry_point_declared_exported_abi6(lib):
     from gaussianhaircut_b200 import _capi, losses
     src = open(os.path.join(ROOT, "include", "gh_rasterizer.h")).read()
     assert re.search(r"\bint gh_image_loss_stage\s*\(int width, int height, int stage, unsigned options,", src)
@@ -207,7 +207,7 @@ def test_stage_entry_point_declared_exported_abi5(lib):
     assert (losses.ORIENT_UNIT_WEIGHT, losses.ORIENT_NO_CONF) == (sl.UNIT_WEIGHT, sl.NO_CONF) == (1, 2)
     assert hasattr(lib, "gh_image_loss_stage") and "gh_image_loss_stage" in _capi.SIGNATURES
     assert len(_capi.SIGNATURES["gh_image_loss_stage"][1]) == 18
-    assert lib.gh_abi_version() == 5 and _capi.ABI_VERSION == 5
+    assert lib.gh_abi_version() == 6 and _capi.ABI_VERSION == 6
 
 
 def test_python_layer_rejects_without_a_device():

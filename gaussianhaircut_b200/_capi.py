@@ -92,6 +92,9 @@ SIGNATURES = {
     "gh_render_maps": (_i, [_i, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),   # W H out_color angle conf_masked render hair head orient orient_vis conf_vis stream
     "gh_eval_metrics_workspace_size": (_i, [_i, _i, C.POINTER(_sz)]),
     "gh_eval_metrics": (_i, [_i, _i, _i, _p, _p, _p, _p, _p, _p, _sz, _p, _p]),   # W H stage out_color gt_image gt_mask gt_angle gt_conf workspace bytes row stream
+    "gh_eval_ssim_workspace_size": (_i, [_i, _i, _i, C.POINTER(_sz)]),   # B W H bytes
+    "gh_eval_ssim": (_i, [_i, _i, _i, _p, _i, _ll, _p, _i, _ll, _p, _ll, C.c_uint, _p, _ll, _p, _ll, _p, _sz, _i, _p]),
+    # B W H img1 dtype1 stride1 img2 dtype2 stride2 mask mask_stride flags ssim ssim_stride psnr psnr_stride workspace bytes debug stream
     "gh_project_workspace_size": (_i, [_i, C.POINTER(C.c_size_t)]),
     "gh_project_forward": (_i, _PROJ_ARGS + [
         _p, _p, _p, _p, _p, _p,              # means2D colors opacities conic cov3D visible

@@ -28,7 +28,7 @@
 namespace {
 
 #define GH_LT 32                       // loss tile edge (pixels); 256 threads, 4 pixels each
-#define GH_LR 5                        // window radius: 11 taps
+#define GH_LR GH_SSIM_R                // window radius: 11 taps
 #define GH_LH (GH_LT + 2 * GH_LR)      // halo tile edge: 42
 #define GH_XS (GH_LH + 1)              // row stride of the halo arrays (float2): conflict-free column walks
 #define GH_HS (GH_LT + 1)              // row stride of the horizontally filtered arrays
@@ -219,7 +219,6 @@ gh_loss_main_kernel(GhLossParams prm, const float* __restrict__ out, const float
     const int tid = threadIdx.x;
 
     // ------------------------------------------------------------------ SSIM statistics, channel by channel
-    const float C1 = 0.01f * 0.01f, C2 = 0.03f * 0.03f;
     double a_ssim = 0.0;
     for (int c = 0; c < 3; c++) {
         __syncthreads();
@@ -314,12 +313,8 @@ gh_loss_main_kernel(GhLossParams prm, const float* __restrict__ out, const float
                 if (px < W && py < H) {
                     const int pi = py * W + px;
                     const float mu1 = m.x, mu2 = m.y;
-                    const float mu1_sq = mu1 * mu1, mu2_sq = mu2 * mu2, mu12 = mu1 * mu2;
-                    const float sg1 = e.x - mu1_sq, sg2 = e.y - mu2_sq, sg12 = e12 - mu12;
-                    const float a1 = 2.f * mu12 + C1, a2 = 2.f * sg12 + C2;
-                    const float b1 = mu1_sq + mu2_sq + C1, b2 = sg1 + sg2 + C2;
-                    const float ib = __frcp_rn(b1 * b2);
-                    const float S = a1 * a2 * ib;
+                    const GhSsimPixel sp = gh_ssim_pixel(mu1, mu2, e.x, e.y, e12);
+                    const float a1 = sp.a1, a2 = sp.a2, b1 = sp.b1, b2 = sp.b2, ib = sp.ib, S = sp.S;
                     a_ssim += (double)S;
                     // derivatives of the map w.r.t. conv(x), conv(x^2), conv(x y) at this pixel
                     float* dm = dmaps + (size_t)c * 3 * (size_t)plane;
@@ -555,11 +550,7 @@ int gh_image_loss_run(const char* who, int width, int height, int stage, unsigne
     GhLossParams prm;
     prm.W = width; prm.H = height;
     prm.l_dl1 = lambda_dl1; prm.l_dssim = lambda_dssim; prm.l_dmask = lambda_dmask; prm.l_dorient = lambda_dorient;
-    {   // gaussian(11, 1.5) as the reference builds it: float32 taps, float32 normalisation
-        float g[11], sum = 0.f;
-        for (int k = 0; k < 11; k++) { g[k] = (float)exp(-(double)((k - 5) * (k - 5)) / (2.0 * 1.5 * 1.5)); sum += g[k]; }
-        for (int k = 0; k < 11; k++) prm.g[k] = g[k] / sum;
-    }
+    gh_ssim_window(prm.g);
     double* sums = reinterpret_cast<double*>(workspace);
     const cudaError_t e = cudaMemsetAsync(sums, 0, GH_LS_COUNT * sizeof(double), stream);     // sums + tickets
     if (e != cudaSuccess) return gh_cuda_status(who, "memset(partial sums)", e);

@@ -10,7 +10,8 @@
 paths (DESIGN.md §16/§19/§20) with the binning capacity carried from view to view (it starts at 0: the first view
 is rendered twice).  `gh_render_maps` turns the raw
 (10,H,W) image into the maps the scripts save -- the bytes of `torchvision.utils.save_image` included -- in one kernel,
-`gh_eval_metrics` into the numbers `training_report` prints.  There is no CPU path: CPU tensors raise.
+`gh_eval_metrics` into the numbers `training_report` prints, and `gh_eval_ssim` (`eval_ssim`, `evaluate_views(...,
+ssim=True)`) adds the SSIM of loss_utils.ssim.  There is no CPU path: CPU tensors raise.
 """
 from __future__ import annotations
 
@@ -27,7 +28,7 @@ from .graphs import STATUS_BINNING_OVERFLOW
 from .losses import STAGES
 
 __all__ = ["ViewRenderer", "sweep", "write_render_set", "maps_to_supervision", "evaluate_views", "eval_metrics",
-           "MAP_NAMES", "RENDER_SET_MAPS", "METRIC_NAMES"]
+           "eval_ssim", "MAP_NAMES", "RENDER_SET_MAPS", "METRIC_NAMES"]
 
 # gh_render_maps' outputs in argument order: name -> (dtype, trailing shape after (H, W); floats are (1,H,W))
 MAP_NAMES = ("orient_angle", "orient_conf_masked", "render_u8", "hair_mask_u8", "head_mask_u8", "orient_u8",
@@ -420,18 +421,105 @@ def eval_metrics(raw: torch.Tensor, gt_image: torch.Tensor, gt_mask: torch.Tenso
                                                  _stream(dev)))
 
 
+def ssim_workspace(B: int, W: int, H: int, device: torch.device) -> torch.Tensor:
+    nbytes = C.c_size_t()
+    _capi.check(_capi.load().gh_eval_ssim_workspace_size(int(B), int(W), int(H), C.byref(nbytes)))
+    return torch.empty((nbytes.value + 7) // 8, dtype=torch.float64, device=device)
+
+
+_DTYPES = {torch.float32: 0, torch.uint8: 1}          # GH_DTYPE_FLOAT32, GH_DTYPE_UINT8
+_CLAMP1, _CLAMP2, _CLAMP_MASK = 1, 2, 4               # GH_SSIM_CLAMP_IMG1, _IMG2, _MASK
+
+
+def _pairs(t: torch.Tensor, name: str, dev: torch.device, C_: int) -> Tuple[torch.Tensor, int]:
+    """`t` as B planar (C_,H,W) blocks: (B,C_,H,W), or (C_,H,W) for B = 1; each block contiguous, the pair stride free
+    (so raw[:3] of a (10,H,W) render or x[:, :3] of a (B,10,H,W) stack is read in place).  -> (tensor, pair stride)."""
+    if not t.is_cuda:
+        raise RuntimeError(f"eval_ssim: '{name}' must be a CUDA tensor (there is no CPU path)")
+    if t.device != dev:
+        raise RuntimeError(f"eval_ssim: '{name}' is on {t.device}, expected {dev}")
+    if t.dim() == 3:
+        t = t.unsqueeze(0)
+    if t.dim() != 4 or t.shape[1] != C_:
+        raise RuntimeError(f"eval_ssim: '{name}' must have shape (B,{C_},H,W) or ({C_},H,W), got {tuple(t.shape)}")
+    if t.requires_grad:
+        t = t.detach()
+    H, W = int(t.shape[2]), int(t.shape[3])
+    if t.stride()[1:] != (H * W, W, 1) and not (C_ == 1 and t.stride()[2:] == (W, 1)):
+        t = t.contiguous()
+    if t.data_ptr() % t.element_size():
+        t = t.clone()
+    return t, (int(t.stride(0)) if t.shape[0] > 1 else C_ * H * W)
+
+
+def _out_vec(t: Optional[torch.Tensor], name: str, B: int, dev: torch.device) -> Tuple[Optional[torch.Tensor], int]:
+    if t is None:
+        return None, 0
+    if t.dtype != torch.float32 or t.dim() != 1 or t.numel() != B or t.device != dev:
+        raise RuntimeError(f"eval_ssim: {name} must be a float32 ({B},) tensor on {dev} (any stride, e.g. rows[:, 4])")
+    return t, int(t.stride(0))
+
+
+def eval_ssim(img1: torch.Tensor, img2: torch.Tensor, out_ssim: torch.Tensor, out_psnr: Optional[torch.Tensor] = None,
+              clamp1: bool = False, mask: Optional[torch.Tensor] = None, workspace: Optional[torch.Tensor] = None,
+              clamp2: bool = False, clamp_mask: bool = False, debug: bool = False) -> None:
+    """gh_eval_ssim: loss_utils.ssim(img1[i], img2[i]) into out_ssim[i] and image_utils.psnr(img1[i], img2[i]) into
+    out_psnr[i] (optional) for B pairs, in one launch.
+
+    img1, img2: (B,3,H,W) or (3,H,W) device tensors, float32 or uint8 (x / 255 as torchvision's to_tensor rounds it; a
+    uint8 image and its to_tensor conversion give the same bits); each (3,H,W) block contiguous, the pair stride free.
+    clamp1 / clamp2 clamp that image to [0, 1].  mask: (B,1,H,W) or (1,H,W) float32, multiplied into both images
+    (clamped to [0, 1] first with clamp_mask).  out_ssim, out_psnr: float32 (B,) device tensors of any stride, such as
+    rows[:, 4] and rows[:, 3] of an (N,8) metrics buffer.  workspace: ssim_workspace(B, W, H, device) or None.
+    No host synchronisation (unless debug)."""
+    dev = img1.device
+    for name, t in (("img1", img1), ("img2", img2)):
+        if t.dtype not in _DTYPES:
+            raise RuntimeError(f"eval_ssim: '{name}' must be float32 or uint8, got {t.dtype}")
+    a, s1 = _pairs(img1, "img1", dev, 3)
+    b, s2 = _pairs(img2, "img2", dev, 3)
+    if a.shape != b.shape:
+        raise RuntimeError(f"eval_ssim: img1 {tuple(a.shape)} and img2 {tuple(b.shape)} differ")
+    B, H, W = int(a.shape[0]), int(a.shape[2]), int(a.shape[3])
+    sm = 0
+    if mask is not None:
+        if mask.dtype != torch.float32:
+            raise RuntimeError(f"eval_ssim: mask must be float32, got {mask.dtype}")
+        mask, sm = _pairs(mask, "mask", dev, 1)
+        if tuple(mask.shape) != (B, 1, H, W):
+            raise RuntimeError(f"eval_ssim: mask must have shape {(B, 1, H, W)}, got {tuple(mask.shape)}")
+    o_s, ss = _out_vec(out_ssim, "out_ssim", B, dev)
+    if o_s is None:
+        raise RuntimeError("eval_ssim: out_ssim is required")
+    o_p, sp = _out_vec(out_psnr, "out_psnr", B, dev)
+    if workspace is None:
+        workspace = ssim_workspace(B, W, H, dev)
+    flags = (_CLAMP1 if clamp1 else 0) | (_CLAMP2 if clamp2 else 0) | (_CLAMP_MASK if clamp_mask else 0)
+    with torch.cuda.device(dev):
+        _capi.check(_capi.load().gh_eval_ssim(B, W, H, _ptr(a), _DTYPES[a.dtype], s1, _ptr(b), _DTYPES[b.dtype], s2,
+                                              _ptr(mask), sm, flags, _ptr(o_s), ss, _ptr(o_p), sp, _ptr(workspace),
+                                              workspace.numel() * workspace.element_size(), int(bool(debug)),
+                                              _stream(dev)))
+
+
 def _gt_of(view, dev):
     g = lambda t: t.to(dev, non_blocking=True)  # noqa: E731
     return g(view.original_image), g(view.original_mask), g(view.original_orient_angle), g(view.original_orient_conf)
 
 
-def evaluate_views(views, view_renderer: ViewRenderer, stage: str) -> Dict[str, float]:
+def evaluate_views(views, view_renderer: ViewRenderer, stage: str, ssim: bool = False) -> Dict[str, float]:
     """training_report's loop over `views` (src/train_gaussians.py:246-281 and the strand trainers' copies): per view the
     ground truth maps go to the device (`original_image`, `original_mask`, `original_orient_angle`,
     `original_orient_conf`), the view is rendered and gh_eval_metrics fills row i of an (N,8) device buffer; the buffer
     and the views' status words are read back once after the last view, an overflowed view is redone, and the means
     over the views are taken in float64 on the host.  -> {"l1", "mask" ("ce" in the latent strand stage), "or", "psnr"}
-    plus "mse_r", "mse_g", "mse_b"."""
+    plus "mse_r", "mse_g", "mse_b".
+
+    ssim=True adds "ssim": gh_eval_ssim writes slot 4 of each row, on the same stream after gh_eval_metrics, from the
+    pair the row's l1 term uses -- the render's image channels and gt_image, both clamped to [0, 1], and in the
+    latent strand stage both multiplied by the clamped gt_mask[:1].  The other slots are the same bits as without it."""
+    if not isinstance(ssim, bool):
+        raise TypeError(f"evaluate_views: ssim must be True or False, got {ssim!r}")
     views = list(views)
     if not views:
         return {}
@@ -444,8 +532,13 @@ def evaluate_views(views, view_renderer: ViewRenderer, stage: str) -> Dict[str, 
         nonlocal ws
         raw = view_renderer.render_raw(view, check=check)
         if ws is None or ws[0] != tuple(raw.shape):
-            ws = (tuple(raw.shape), eval_workspace(int(raw.shape[2]), int(raw.shape[1]), dev))
-        eval_metrics(raw, *_gt_of(view, dev), stage, rows[i], ws[1])
+            H, W = int(raw.shape[1]), int(raw.shape[2])
+            ws = (tuple(raw.shape), eval_workspace(W, H, dev), ssim_workspace(1, W, H, dev) if ssim else None)
+        gts = _gt_of(view, dev)
+        eval_metrics(raw, *gts, stage, rows[i], ws[1])
+        if ssim:
+            eval_ssim(raw[:3], gts[0], rows[i, 4:5], clamp1=True, clamp2=True, workspace=ws[2],
+                      mask=gts[1][:1] if stage == "latent_strands" else None, clamp_mask=True)
         ios[i].copy_(view_renderer.io)
 
     for i, view in enumerate(views):
@@ -459,4 +552,4 @@ def evaluate_views(views, view_renderer: ViewRenderer, stage: str) -> Dict[str, 
     names = list(METRIC_NAMES)
     if stage == "latent_strands":
         names[1] = "ce"
-    return {k: float(m[j]) for j, k in enumerate(names) if k != "ssim"}
+    return {k: float(m[j]) for j, k in enumerate(names) if k != "ssim" or ssim}

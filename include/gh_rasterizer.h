@@ -319,6 +319,42 @@ int gh_eval_metrics(int width, int height, int stage, const float* out_color, co
                     void* workspace, size_t workspace_bytes, float* row, gh_stream_t stream);
 
 /*
+ * SSIM and PSNR of B image pairs, forward only (src/metrics.py):
+ *   ssim[i] = loss_utils.ssim(img1[i], img2[i]) with size_average: the 11x11 Gaussian window (sigma 1.5, float32 1-D
+ *     taps as create_window builds them, applied separably), zero padding 5, C1 = 0.01^2, C2 = 0.03^2, the mean of
+ *     ssim_map over 3 H W;
+ *   psnr[i] = image_utils.psnr on a (1,3,H,W) image: 20 log10(1 / sqrt(mse)) with one mse over all 3 H W values
+ *     (mse 0 gives +inf).
+ * img1, img2: B pairs of planar (3,H,W) images (channel stride H W), pair i at element offset i * stride1 / stride2 --
+ *   so a stack of raw (10,H,W) renders is read in place with stride 10 H W.  dtype GH_DTYPE_FLOAT32, or
+ *   GH_DTYPE_UINT8 read as x / 255 rounded as torchvision's to_tensor rounds it: a uint8 pair and its float32
+ *   conversion give the same bits.  flags: GH_SSIM_CLAMP_IMG1 / _IMG2 clamp that image to [0,1] after conversion (what
+ *   training_report does to a render and its ground truth).  mask: NULL, or per pair a float32 (1,H,W) multiplier at
+ *   offset i * mask_stride applied to both images (the latent strand stage's gt_mask[:1]), clamped to [0,1] with
+ *   GH_SSIM_CLAMP_MASK.
+ * ssim (device float, pair i at i * ssim_stride) is required, psnr (same layout) optional: NULL skips it.  Pointing
+ *   them into slot 4 / 3 of an (N,8) gh_eval_metrics row buffer takes stride 8.
+ * Sums are per-pixel terms in double, per CTA through a fixed-order block sum, the CTAs of a pair added in CTA order:
+ *   the results are bit-identical run to run, and pair i's bits do not depend on B or on the other pairs.
+ * workspace: gh_eval_ssim_workspace_size(B, W, H) bytes, 8-byte aligned.  debug != 0 synchronises after the launches
+ * and reports a failure there.  Three stream operations (memset + 2 launches), no allocation, no host synchronisation
+ * (unless debug).  Refused (GH_E_INVALID_ARG, before any CUDA call): B, W or H <= 0, B > 65535, B 3 H W or the strided
+ * extent beyond 2^31 - 1 elements, overlapping pair strides, an unknown dtype code or flag bit, a NULL image, ssim or
+ * workspace pointer, misaligned float arrays, a workspace that is misaligned or smaller than the size query's, and
+ * debug != 0 while the stage timer is on.
+ */
+#define GH_DTYPE_FLOAT32 0
+#define GH_DTYPE_UINT8   1
+#define GH_SSIM_CLAMP_IMG1 1u
+#define GH_SSIM_CLAMP_IMG2 2u
+#define GH_SSIM_CLAMP_MASK 4u
+int gh_eval_ssim_workspace_size(int B, int width, int height, size_t* bytes);
+int gh_eval_ssim(int B, int width, int height, const void* img1, int dtype1, long long stride1,
+                 const void* img2, int dtype2, long long stride2, const float* mask, long long mask_stride,
+                 unsigned flags, float* ssim, long long ssim_stride, float* psnr, long long psnr_stride,
+                 void* workspace, size_t workspace_bytes, int debug, gh_stream_t stream);
+
+/*
  * Multi-GPU (SURVEY.md 8e): sum a float32 buffer that lives in SYMMETRIC memory (the same allocation on
  * every GPU of the node, each mapped into every process, e.g. torch.distributed._symmetric_memory) over
  * all ranks, in place, with one kernel per rank that reads and writes its peers' copies through NVLink.

@@ -175,6 +175,9 @@ SIGNATURES = {
     "gh_camera_forward": (_i, [_i, _p, _p, _p, _p, _p, _p, _p, _p, _i, _p]),   # n residuals base index view proj campos tan status debug stream
     "gh_camera_backward": (_i, [_i, _p, _p, _p, _i, _p, _p, _p, _p, _p, _i, _p]),   # n residuals base index intrinsics d_camera grad touched nan status debug stream
     "gh_camera_adam_step": (_i, [_i, _i, _p, _p, _p, _p, _p, _p, _p, _d, _d, _f, _p, _p, _i, _p]),   # n intrinsics r grad touched m v steps lrs b1 b2 eps nan skip debug stream
+    "gh_sdf_workspace_size": (_i, [_ll, C.POINTER(_sz)]),                    # F bytes
+    "gh_sdf_prepare": (_i, [_ll, _ll, _p, _p, _p, _sz, _p, _i, _p]),       # V F verts faces workspace bytes status debug stream
+    "gh_sdf_query": (_i, [_ll, _p, _ll, _p, _sz, _p, _p, _p, _i, _p]),     # N points F workspace bytes sdf dist winding debug stream
 }
 
 _lib = None

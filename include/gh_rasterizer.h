@@ -752,6 +752,37 @@ int gh_orient_dog(int H, int W, int C, const unsigned char* image, const double*
 int gh_orient_gabor(int H, int W, const float* bank, int N, int K, int num_filters, const float* thetas,
                     long long* orients, float* var, void* workspace, size_t bytes, gh_stream_t stream);
 
+/*
+ * Signed distance of points to a triangle mesh (the reference's `pysdf.SDF`, called by
+ * src/preprocessing/filter_flame_intersections.py:115-118 and export_curves.py:41; DESIGN §23).  Mesh: V vertices
+ * (V,3) float32 and F faces (F,3) int32; queries: N points (N,3) float32.
+ *   d(p)   = Euclidean distance from p to the closest point of the union of the F triangles; a degenerate triangle
+ *            counts as its segment or point;
+ *   w(p)   = generalized winding number sum_f Omega_f(p) / 4 pi, Omega_f the signed solid angle of triangle f (Van
+ *            Oosterom-Strackee, 2 atan2(A . (B x C), |A||B||C| + (A.B)|C| + (A.C)|B| + (B.C)|A|), A = a - p, ...):
+ *            1 inside and 0 outside a closed, consistently (counter-clockwise seen from outside) oriented mesh, smooth
+ *            across the holes of an open one;
+ *   sdf(p) = +d if w > 0.5, else -d: positive inside (sdf < 0 is outside, as the reference reads it).
+ * A query with a NaN or infinite coordinate gets NaN in every output.  Each result depends only on its point and the
+ * mesh, visited in face order: results are bit-reproducible and independent of N and of the launch shape.
+ * Two calls on one stream, sharing a workspace of gh_sdf_workspace_size(F) bytes (16-byte aligned device memory):
+ *   gh_sdf_prepare reads verts and faces once and writes one record per face (gaussianhaircut_b200/csrc/
+ *     gh_mesh_math.h).  A face index outside [0, V) ORs GH_STATUS_SDF_FACE_INDEX into *status (device, zeroed by the
+ *     caller) and gives that face a NaN record: nothing out of range is read, and query results are then unspecified.
+ *   gh_sdf_query: one brute-force pass over every face for every point; sdf (N) float32 required, dist and winding
+ *     (N) float32 optional (NULL skips them).  N = 0 launches nothing.
+ * debug != 0 synchronises after the launch and reports a failure there.  No allocation, no host synchronisation
+ * (unless debug).  Refused (GH_E_INVALID_ARG, before any CUDA call): V, F <= 0, N < 0, any of them above 2^31 - 1, a
+ * NULL or misaligned pointer (float and int arrays 4-byte, workspace 16-byte), a workspace smaller than the size
+ * query's, and debug != 0 while the stage timer is on.
+ */
+#define GH_STATUS_SDF_FACE_INDEX 4u
+int gh_sdf_workspace_size(long long F, size_t* bytes);
+int gh_sdf_prepare(long long V, long long F, const float* verts, const int* faces, void* workspace, size_t bytes,
+                   unsigned int* status, int debug, gh_stream_t stream);
+int gh_sdf_query(long long N, const float* points, long long F, const void* workspace, size_t bytes, float* sdf,
+                 float* dist, float* winding, int debug, gh_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

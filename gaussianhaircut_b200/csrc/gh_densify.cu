@@ -12,13 +12,16 @@
 //             split = g >= thr and s_max >  percent_dense * extent        (:687-689; clones have padded grad 0)
 //             the final prune (:728-733) per resulting row: opacity < min_opacity, or world-size s_max > 0.1 * extent
 //             (the screen-size test never fires: densification_postfix zeroes max_radii2D before it is read, :674);
-//             children of a split use the shrunk scale s / (0.8 * 2)      (:695)
+//             children of a split use the shrunk scale s / (0.8 * 2)      (:695), which torch on the device forms as
+//             s * fl(1 / fl(1.6)) = s * 0.625f (a tensor divided by a Python scalar is multiplied by its reciprocal);
+//             s_max and the children's max are NaN when any component is, as torch.max is: no NaN row is cloned,
+//             split or pruned on its size
 //             -> keep flags A (original survives: not split, not pruned), B (its clone survives), C (its two children survive)
 //   scan      exclusive prefix sums of the three flags (device-wide; done by the caller)
 //   scatter   (one thread per source Gaussian): rows go to their final position in the reference's order
 //             [surviving originals | surviving clones | first children | second children], parameters and both Adam
 //             moments in the same pass; clones and children start with zero moments (:640-641); child position =
-//             R(q) * sample + xyz with the caller's N(0, s) samples (:690-694), child log-scale = log(s / 1.6).
+//             R(q) * sample + xyz with the caller's N(0, s) samples (:690-694), child log-scale = log(s * 0.625f).
 // Everything is written exactly once; nothing is re-allocated in between.
 #include "gh_common.cuh"
 #include "gh_kernels.h"
@@ -40,6 +43,12 @@ struct GhDensifyTensors {
     int xyz_index, scaling_index, rotation_index;
 };
 
+// torch.max(dim=1) propagates a NaN component; fmaxf would drop it
+__device__ __forceinline__ float gh_max_nan(float a, float b) { return (a != a || a > b) ? a : b; }
+
+// a split child's scale, get_scaling / (0.8 * 2), bit-identical to torch's s * (1.0f / 1.6f) with 1.0f / 1.6f = 0.625f
+__device__ __forceinline__ float gh_child_scale(float s) { return s * 0.625f; }
+
 __global__ void __launch_bounds__(256)
 gh_densify_classify_kernel(int P, const float* __restrict__ grad_accum, const float* __restrict__ denom,
                            const float* __restrict__ log_scaling, const float* __restrict__ opacity_logit,
@@ -51,14 +60,14 @@ gh_densify_classify_kernel(int P, const float* __restrict__ grad_accum, const fl
     float g = grad_accum[i] / denom[i];
     if (g != g) g = 0.f;                                               // grads[grads.isnan()] = 0.0
     const float s0 = expf(log_scaling[3 * (size_t)i]), s1 = expf(log_scaling[3 * (size_t)i + 1]), s2 = expf(log_scaling[3 * (size_t)i + 2]);
-    const float smax = fmaxf(s0, fmaxf(s1, s2));
+    const float smax = gh_max_nan(s0, gh_max_nan(s1, s2));
     const bool hot = (fabsf(g) >= grad_threshold);
     const bool clone = hot && (smax <= dense_extent);
     const bool split = (g >= grad_threshold) && (smax > dense_extent);
     const float op = 1.0f / (1.0f + expf(-opacity_logit[i]));
     const bool prune_self = (op < min_opacity) || (ws_limit > 0.f && smax > ws_limit);
-    // children: new log-scale = log(s / 1.6); their get_scaling is exp(log(s / 1.6))
-    const float cmax = fmaxf(expf(logf(s0 / 1.6f)), fmaxf(expf(logf(s1 / 1.6f)), expf(logf(s2 / 1.6f))));
+    // children: new log-scale = log(s * 0.625f); their get_scaling is exp of that
+    const float cmax = gh_max_nan(expf(logf(gh_child_scale(s0))), gh_max_nan(expf(logf(gh_child_scale(s1))), expf(logf(gh_child_scale(s2)))));
     const bool prune_child = (op < min_opacity) || (ws_limit > 0.f && cmax > ws_limit);
     reinterpret_cast<int4*>(flags)[i] = make_int4((!split && !prune_self) ? 1 : 0, (clone && !prune_self) ? 1 : 0,
                                                   (split && !prune_child) ? 1 : 0, split ? 1 : 0);
@@ -101,7 +110,7 @@ gh_densify_scatter_kernel(int P, GhDensifyTensors T, const int* __restrict__ fla
         child1[1] = R10 * sB[0] + R11 * sB[1] + R12 * sB[2] + x[1];
         child1[2] = R20 * sB[0] + R21 * sB[1] + R22 * sB[2] + x[2];
 #pragma unroll
-        for (int k = 0; k < 3; k++) cscale[k] = logf(expf(ls[k]) / 1.6f);     // scaling_inverse_activation(get_scaling / (0.8 * N))
+        for (int k = 0; k < 3; k++) cscale[k] = logf(gh_child_scale(expf(ls[k])));   // scaling_inverse_activation(get_scaling / (0.8 * N))
     }
     for (int t = 0; t < T.n; t++) {
         const int row = T.row[t];

@@ -689,7 +689,9 @@ int gh_strand_backward(int S, int L, const float* d_xyz, float* d_dirs, unsigned
  *   samples (2 * n_split_all, 3): N(0, scale) draws, first-children block then second-children block
  *   (torch.normal(mean=0, std=get_scaling[mask].repeat(2, 1)), :690-692).  Destination rows follow the reference's
  *   order [surviving originals | surviving clones | first children | second children]; clones and children get zero
- *   moments; child xyz = R(q) sample + xyz, child log-scale = log(scale / 1.6).
+ *   moments; child xyz = R(q) sample + xyz, child log-scale = log(scale * 0.625f), the float32 product torch forms for
+ *   scale / (0.8 * 2) on the device.  A NaN log-scale component makes the row's max scale NaN (torch.max), so the
+ *   row is neither cloned, split nor pruned on its size.
  */
 int gh_densify_classify(int P, const float* grad_accum, const float* denom, const float* log_scaling,
                         const float* opacity_logit, float grad_threshold, float dense_extent,

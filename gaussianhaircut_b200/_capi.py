@@ -178,6 +178,9 @@ SIGNATURES = {
     "gh_sdf_workspace_size": (_i, [_ll, C.POINTER(_sz)]),                    # F bytes
     "gh_sdf_prepare": (_i, [_ll, _ll, _p, _p, _p, _sz, _p, _i, _p]),       # V F verts faces workspace bytes status debug stream
     "gh_sdf_query": (_i, [_ll, _p, _ll, _p, _sz, _p, _p, _p, _i, _p]),     # N points F workspace bytes sdf dist winding debug stream
+    "gh_mesh_raster_workspace_size": (_i, [_ll, _ll, _i, _i, _i, C.POINTER(_sz)]),   # V F H W chunk bytes
+    "gh_mesh_raster": (_i, [_ll, _ll, _p, _p, _i, _p, _p, _p, _i, _i, _p, _p, _p, _p, _p, _i, _p, _sz, _p, _i, _p]),
+    # V F verts faces B K R t H W head_mask pix_to_face vis_head vis_count vis_count_head chunk workspace bytes status debug stream
 }
 
 _lib = None

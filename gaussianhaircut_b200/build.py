@@ -19,7 +19,7 @@ OBJ_DIR = os.path.join(LIB_DIR, "obj")
 LIB_PATH = os.path.join(LIB_DIR, "libgh_raster.so")
 INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 
-SOURCES = ["gh_api.cu", "gh_preprocess.cu", "gh_binning.cu", "gh_blend.cu", "gh_preprocess_bwd.cu", "gh_adam.cu", "gh_image_loss.cu", "gh_allreduce.cu", "gh_project.cu", "gh_densify.cu", "gh_strands.cu", "gh_knn.cu", "gh_orient.cu", "gh_camera.cu", "gh_render_maps.cu", "gh_eval_ssim.cu", "gh_sdf.cu"]
+SOURCES = ["gh_api.cu", "gh_preprocess.cu", "gh_binning.cu", "gh_blend.cu", "gh_preprocess_bwd.cu", "gh_adam.cu", "gh_image_loss.cu", "gh_allreduce.cu", "gh_project.cu", "gh_densify.cu", "gh_strands.cu", "gh_knn.cu", "gh_orient.cu", "gh_camera.cu", "gh_render_maps.cu", "gh_eval_ssim.cu", "gh_sdf.cu", "gh_mesh_raster.cu"]
 HEADERS = ["gh_common.cuh", "gh_kernels.h", "gh_project_math.h", "gh_knn_math.h", "gh_orient_math.h", "gh_adam_math.cuh", "gh_camera_math.h", "gh_image_math.cuh", "gh_mesh_math.h"]
 
 NVCC_FLAGS = [

@@ -28,7 +28,7 @@ gh_sdf_prepare_kernel(int V, int F, const float* __restrict__ verts, const int* 
     if (f >= F) return;
     const int i0 = __ldg(faces + 3 * (size_t)f), i1 = __ldg(faces + 3 * (size_t)f + 1), i2 = __ldg(faces + 3 * (size_t)f + 2);
     GhSdfRecord r;
-    if (i0 < 0 || i0 >= V || i1 < 0 || i1 >= V || i2 < 0 || i2 >= V) {
+    if (!gh_mesh_face_in_range(i0, i1, i2, V)) {
         atomicOr(status, GH_STATUS_SDF_FACE_INDEX);
         for (int k = 0; k < 28; k++) r.v[k] = __int_as_float(0x7fffffff);
     } else {

@@ -4,19 +4,29 @@
 `MeshSDF(verts, faces)(points)` = +d inside, -d outside, d the distance to the closest point of the mesh and the side
 decided by the generalized winding number (contract: include/gh_rasterizer.h; kernels: csrc/gh_sdf.cu).
 `flame_filter_keep` is lines 88 and 104-119 of the script: the mask of Gaussians that `prune_points` keeps, built on
-the device with no host copy.  Nothing here loads the native library or touches CUDA until it is called.
+the device with no host copy.
+
+The head mesh rasterized per view, what `src/preprocessing/extract_non_visible_head_scalp.py` gets from pytorch3d's
+`MeshRasterizer` (DESIGN §24): `rasterize_faces` (a z-buffered `pix_to_face`), `head_masks` (the script's dilated
+hair/body masks) and `scalp_visibility` (its `check_visiblity_of_faces`).  Kernels: csrc/gh_mesh_raster.cu.
+
+Nothing here loads the native library or touches CUDA until it is called.
 """
 from __future__ import annotations
 
 import ctypes as C
 import math
+import warnings
 
 import torch
+import torch.nn.functional as Fn
 
 from . import _capi
 from ._capi import _ptr, _stream
 
 GH_STATUS_SDF_FACE_INDEX = 4        # include/gh_rasterizer.h
+GH_STATUS_RASTER_NEAR = 8
+RASTER_ZBUF_BYTES = 1 << 30          # the z-buffer share of rasterize_faces' workspace: it sets the views per chunk
 
 
 class MeshSDF:
@@ -127,3 +137,127 @@ def flame_filter_keep(xyz: torch.Tensor, scaling: torch.Tensor, rotation: torch.
     corners = flame_corners(xyz.detach(), scaling.detach(), rotation.detach())
     outside = (sdf(corners).view(xyz.shape[0], 12) < 0).all(dim=1)
     return torch.logical_or(outside, label.detach().squeeze() <= 0.5)
+
+
+def _raster_args(verts, faces, K, R, t, H, W):
+    if verts.dim() != 2 or verts.shape[1] != 3 or faces.dim() != 2 or faces.shape[1] != 3:
+        raise RuntimeError(f"mesh raster: verts and faces must be (V, 3) and (F, 3), got {tuple(verts.shape)} and "
+                           f"{tuple(faces.shape)}")
+    if faces.dtype != torch.int32:
+        raise RuntimeError(f"expected scalar type Int but found {faces.dtype} for argument 'faces'")
+    if verts.shape[0] < 1 or faces.shape[0] < 1:
+        raise RuntimeError("mesh raster: the mesh needs at least one vertex and one face")
+    B = K.shape[0] if K.dim() == 3 else -1
+    for name, x, shape in (("K", K, (B, 3, 3)), ("R", R, (B, 3, 3)), ("t", t, (B, 3))):
+        if tuple(x.shape) != shape or B < 1:
+            raise RuntimeError(f"mesh raster: '{name}' must have shape (B, {', '.join(map(str, shape[1:]))}) with one "
+                               f"B >= 1 for K, R and t, got {tuple(x.shape)}")
+    if not (1 <= int(H) <= 8192 and 1 <= int(W) <= 8192):
+        raise RuntimeError(f"mesh raster: H and W must lie in [1, 8192], got {H} x {W}")
+    if not (verts.is_cuda and faces.is_cuda):
+        raise RuntimeError("mesh raster: verts and faces must be CUDA tensors (there is no CPU path)")
+    dev = verts.device
+    if faces.device != dev:
+        raise RuntimeError(f"mesh raster: verts on {dev}, faces on {faces.device}")
+    f32 = [_capi._f32(x, n, dev) for x, n in ((verts, "verts"), (K, "K"), (R, "R"), (t, "t"))]
+    return dev, B, f32, faces.contiguous()
+
+
+def _raster(verts, faces, K, R, t, H, W, chunk, head=None, pix_to_face=None, vis_head=None, counts=None):
+    """One gh_mesh_raster sweep on the current stream; -> the device status word (not read here)."""
+    dev, B, (v, k, r, tt), f = _raster_args(verts, faces, K, R, t, H, W)
+    nv, nf = int(v.shape[0]), int(f.shape[0])
+    lib = _capi.load()
+    nbytes = C.c_size_t()
+    _capi.check(lib.gh_mesh_raster_workspace_size(nv, nf, int(H), int(W), int(chunk), C.byref(nbytes)))
+    with torch.cuda.device(dev):
+        ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+        status = torch.zeros(1, dtype=torch.int32, device=dev)
+        c0, c1 = counts if counts is not None else (None, None)
+        _capi.check(lib.gh_mesh_raster(nv, nf, _ptr(v), _ptr(f), B, _ptr(k), _ptr(r), _ptr(tt), int(H), int(W),
+                                       _ptr(head), _ptr(pix_to_face), _ptr(vis_head), _ptr(c0), _ptr(c1), int(chunk),
+                                       _ptr(ws), nbytes.value, _ptr(status), 0, _stream(dev)))
+    return status
+
+
+def _check_status(status: torch.Tensor, who: str, V: int) -> None:
+    s = int(status.item())
+    if s & GH_STATUS_SDF_FACE_INDEX:
+        raise RuntimeError(f"{who}: a face index lies outside [0, {V})")
+    if s & GH_STATUS_RASTER_NEAR:
+        warnings.warn(f"{who}: a face crosses a camera's z = 0 plane and was skipped (pytorch3d would draw its "
+                      "visible part)", RuntimeWarning, stacklevel=3)
+
+
+def rasterize_faces(verts: torch.Tensor, faces: torch.Tensor, K: torch.Tensor, R: torch.Tensor, t: torch.Tensor,
+                    H: int, W: int) -> torch.Tensor:
+    """pytorch3d's `MeshRasterizer(...)(mesh, cameras=cameras_from_opencv_projection(R, t, K, (H, W))).pix_to_face`
+    with faces_per_pixel = 1 and blur_radius = 0, for B views at once: -> (B, H, W) int32, the covered face of smallest
+    perspective-correct depth at each pixel centre (the smallest index on equal depth), -1 where none is.
+
+    verts (V,3) float32, faces (F,3) int32, K (B,3,3), R (B,3,3), t (B,3) float32, all CUDA tensors on one device; the
+    OpenCV world-to-camera convention, x_cam = R X + t.  The kernels run on the current stream; the status word is
+    read once at the end (one host synchronisation): a face index outside [0, V) raises, and a face that crosses a
+    camera's z = 0 plane -- skipped, where pytorch3d would draw its visible part -- warns."""
+    _raster_args(verts, faces, K, R, t, H, W)
+    B = K.shape[0]
+    chunk = max(1, min(B, RASTER_ZBUF_BYTES // (8 * int(H) * int(W))))
+    out = torch.empty((B, int(H), int(W)), dtype=torch.int32, device=verts.device)
+    status = _raster(verts, faces, K, R, t, H, W, chunk, pix_to_face=out)
+    _check_status(status, "rasterize_faces", int(verts.shape[0]))
+    return out
+
+
+def head_masks(hair: torch.Tensor, body: torch.Tensor) -> torch.Tensor:
+    """extract_non_visible_head_scalp.py:112-115 and 81 on the device: -> bool (B, H, W), True where the dilated body
+    mask is set and the dilated hair mask is not.
+
+    hair, body: uint8 (B, H, W) or (B, H, W, C) images as `cv2.imread` gives them (channel 0 is used, as the script
+    uses it).  `cv2.dilate(m, np.ones((5, 5)))` is a 5x5 max filter that ignores pixels beyond the border: here
+    `max_pool2d` with its -inf padding, exact on integer images.  `dilate / 255. >= 0.5` is `dilate >= 128`, and
+    `clip(body - hair, 0, 1) >= 0.5` is `body and not hair`."""
+    def dilated(m, name):
+        if m.dtype != torch.uint8 or m.dim() not in (3, 4):
+            raise RuntimeError(f"head_masks: '{name}' must be uint8 (B, H, W) or (B, H, W, C), got {m.dtype} "
+                               f"{tuple(m.shape)}")
+        m = m[..., 0] if m.dim() == 4 else m
+        return Fn.max_pool2d(m[:, None].float(), kernel_size=5, stride=1, padding=2)[:, 0] >= 128
+    h, b = dilated(hair, "hair"), dilated(body, "body")
+    if h.shape != b.shape:
+        raise RuntimeError(f"head_masks: hair {tuple(h.shape)} and body {tuple(b.shape)} differ in shape")
+    return b & ~h
+
+
+def scalp_visibility(verts: torch.Tensor, faces: torch.Tensor, K: torch.Tensor, R: torch.Tensor, t: torch.Tensor,
+                     head_masks: torch.Tensor, chunk: int = 16, vis_out: torch.Tensor | None = None):
+    """`check_visiblity_of_faces` (extract_non_visible_head_scalp.py:51-93) for B views: -> (vis_mask bool (V,),
+    vis_maps float32 (V,), vis_maps_head float32 (V,)).
+
+    vis_maps[v] counts the views whose `pix_to_face.unique()[1:]` holds a face of vertex v, vis_maps_head those whose
+    `where(head_mask, pix_to_face, -1).unique()[1:]` does (the kernels count them); then the script's expressions,
+    `prob_hair = 1 - vis_maps_head / vis_maps` and `vis_mask = (prob_hair > 0.5) | (vis_maps / B < 0.1)`, so a vertex
+    no view sees is NaN there and True in vis_mask.  head_masks: bool (B, H, W), one image size for every view, as
+    the script rasterizes every view at one size.  Views run `chunk` at a time (a chunk * H * W * 8-byte z-buffer).
+    vis_out: an optional bool (B, H, W) CUDA tensor that receives the script's per-view images
+    `where(head_mask, pix_to_face, -1) >= 0` from the same pass.  One host synchronisation (the status word)."""
+    if head_masks.dtype != torch.bool or head_masks.dim() != 3:
+        raise RuntimeError(f"scalp_visibility: head_masks must be bool (B, H, W), got {head_masks.dtype} "
+                           f"{tuple(head_masks.shape)}")
+    B, H, W = head_masks.shape
+    if K.dim() != 3 or K.shape[0] != B:
+        raise RuntimeError(f"scalp_visibility: {B} head masks for K of shape {tuple(K.shape)}")
+    if head_masks.device != verts.device:
+        raise RuntimeError(f"scalp_visibility: head_masks on {head_masks.device}, verts on {verts.device}")
+    if vis_out is not None and (vis_out.dtype != torch.bool or tuple(vis_out.shape) != (B, H, W)
+                                or vis_out.device != verts.device or not vis_out.is_contiguous()):
+        raise RuntimeError(f"scalp_visibility: vis_out must be a contiguous bool {(B, H, W)} tensor on {verts.device}")
+    V = int(verts.shape[0])
+    counts = torch.empty((2, V), dtype=torch.int32, device=verts.device)
+    status = _raster(verts, faces, K, R, t, H, W, min(int(chunk), B) if chunk >= 1 else chunk,
+                     head=head_masks.contiguous(), vis_head=vis_out, counts=(counts[0], counts[1]))
+    _check_status(status, "scalp_visibility", V)
+    vis_maps, vis_maps_head = counts[0].float(), counts[1].float()
+    prob_vis_head = vis_maps_head / vis_maps
+    prob_hair = 1 - prob_vis_head
+    vis_mask = torch.logical_or(prob_hair > 0.5, vis_maps / B < 0.1)
+    return vis_mask, vis_maps, vis_maps_head

@@ -785,6 +785,44 @@ int gh_sdf_prepare(long long V, long long F, const float* verts, const int* face
 int gh_sdf_query(long long N, const float* points, long long F, const void* workspace, size_t bytes, float* sdf,
                  float* dist, float* winding, int debug, gh_stream_t stream);
 
+/*
+ * Z-buffered rasterization of one triangle mesh in B views, and the per-vertex visibility counts of the scalp
+ * extraction (pytorch3d's MeshRasterizer with faces_per_pixel = 1, blur_radius = 0, as called by
+ * src/preprocessing/extract_non_visible_head_scalp.py:51-93; DESIGN §24).  Mesh: V vertices (V,3) float32, F faces
+ * (F,3) int32.  Views: K (B,3,3), R (B,3,3) row-major and t (B,3) float32, the OpenCV world-to-camera convention of
+ * cameras_from_opencv_projection: x_cam = R X + t, u = fx x/z + cx, v = fy y/z + cy (only fx, fy, cx, cy of K are
+ * read).  One image size H x W for every view; pixel (row i, column j) samples the point (j + 0.5, i + 0.5).
+ *   coverage: the pixel centre lies strictly inside the projected triangle (all three screen barycentrics > 0: a
+ *     centre on an edge is not covered); back faces are drawn; a zero-area projection never is;
+ *   depth:    the perspective-correct view-space z of the face's plane along the pixel's ray;
+ *   pix_to_face[b,i,j] = the covered face of smallest depth, the smallest index on equal depth, or -1.
+ * Every operation is rounded as gaussianhaircut_b200/csrc/gh_mesh_math.h writes it; a pixel's answer depends only on
+ * the mesh and its camera: bit-reproducible, independent of B, chunk and the launch shape.
+ * Skipped faces (not drawn): a non-finite vertex or projection; all three vertices at view z <= 0; some at z <= 0 and
+ * some in front, which also ORs GH_STATUS_RASTER_NEAR into *status (pytorch3d would draw the visible part); a face
+ * index outside [0, V), which ORs GH_STATUS_SDF_FACE_INDEX into *status and reads nothing out of range.
+ * Outputs (device, any subset, at least one):
+ *   pix_to_face (B,H,W) int32;
+ *   vis_head (B,H,W) uint8 = (head_mask && pix_to_face >= 0), the script's per-view visibility image;
+ *   vis_count, vis_count_head (V) int32, both or neither: per vertex, the number of views whose
+ *     `pix_to_face.unique()[1:]`, respectively that of `where(head_mask, pix_to_face, -1)`, holds a face of the
+ *     vertex.  `[1:]` drops the smallest value: -1 where one occurs, else the smallest face present.
+ * head_mask (B,H,W) uint8 (nonzero = head) is optional: NULL reads as all zero.  Views are processed `chunk` at a time
+ * in a workspace of gh_mesh_raster_workspace_size(V, F, H, W, chunk) bytes (256-byte aligned device memory; it holds a
+ * chunk * H * W * 8-byte z-buffer), so no buffer grows with B.  *status (device) is zeroed by the caller.
+ * debug != 0 synchronises after the launches and reports a failure there.  No allocation, no host synchronisation
+ * (unless debug).  Refused (GH_E_INVALID_ARG, before any CUDA call): V or F outside [1, 2^31), H or W outside
+ * [1, 8192], chunk < 1 or chunk * H * W, chunk * F or chunk * V at or above 2^31, B < 1, a NULL input or status, no
+ * output, only one of the two counts, a misaligned pointer (4-byte for float and int arrays), a missing, misaligned
+ * or short workspace, and debug != 0 while the stage timer is on.
+ */
+#define GH_STATUS_RASTER_NEAR 8u
+int gh_mesh_raster_workspace_size(long long V, long long F, int H, int W, int chunk, size_t* bytes);
+int gh_mesh_raster(long long V, long long F, const float* verts, const int* faces, int B, const float* K,
+                   const float* R, const float* t, int H, int W, const unsigned char* head_mask, int* pix_to_face,
+                   unsigned char* vis_head, int* vis_count, int* vis_count_head, int chunk, void* workspace,
+                   size_t bytes, unsigned int* status, int debug, gh_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

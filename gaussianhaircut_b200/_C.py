@@ -51,11 +51,13 @@ def rasterize_gaussians(
     scale_modifier: float, cov3D_precomp: torch.Tensor, conic_precomp: torch.Tensor,
     viewmatrix: torch.Tensor, projmatrix: torch.Tensor, tan_fovx: float, tan_fovy: float,
     image_height: int, image_width: int, sh: torch.Tensor, degree: int, campos: torch.Tensor,
-    prefiltered: bool, debug: bool,
+    prefiltered: bool, debug: bool, *, zero_records: bool = True,
 ) -> Tuple[int, torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
     """RasterizeGaussiansCUDA (rasterize_points.cu:35-123).
 
     Returns (num_rendered, out_color (C,H,W), radii (P,) int32, geomBuffer, binningBuffer, imgBuffer).
+    `zero_records`: the blend also clears the backward's accumulation records in geomBuffer, so that the first
+    backward on these buffers needs no clearing pass of its own; a caller that runs no backward passes False.
     """
     if means3D.ndim != 2 or means3D.size(1) != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")
@@ -103,7 +105,7 @@ def rasterize_gaussians(
         # (the GPU runs emit from here on if it fitted: keep the host's work until the second phase's launch short)
         R = int(n_rendered.value)
         binningBuffer = _render(background, colors, radii, geomBuffer, imgBuffer, R, int(max_len.value), out_color, debug,
-                                binning if emitted.value else None, stream)
+                                binning if emitted.value else None, stream, zero_records)
         binning_record(key, R)
     return R, out_color, radii, geomBuffer, binningBuffer, imgBuffer
 
@@ -175,24 +177,27 @@ def alloc_forward_workspaces(P: int, W: int, H: int, device: torch.device):
 
 def forward_render(background: torch.Tensor, colors: torch.Tensor, radii: torch.Tensor, geomBuffer: torch.Tensor,
                    imgBuffer: torch.Tensor, num_rendered: int, max_tile_len: int, image_height: int, image_width: int,
-                   debug: bool = False, binned: torch.Tensor | None = None):
+                   debug: bool = False, binned: torch.Tensor | None = None, zero_records: bool = True):
     """Second phase of the forward (emit, sort, blend) on workspaces whose first phase already ran
     (gh_forward_preprocess or gh_project_forward_binned).  `binned`: the binning buffer the first phase already
-    emitted into (projection.project_forward_binned(..., binning=True)); emit is then skipped.
+    emitted into (projection.project_forward_binned(..., binning=True)); emit is then skipped.  `zero_records` as in
+    rasterize_gaussians.
     -> (out_color (C,H,W), binningBuffer)."""
     device = colors.device
     with torch.cuda.device(device):
         out_color = torch.empty((NUM_CHANNELS, int(image_height), int(image_width)), dtype=torch.float32, device=device)
         binningBuffer = _render(_prep(background, "background", device), _prep(colors, "colors", device, align=8), radii,
-                                geomBuffer, imgBuffer, num_rendered, max_tile_len, out_color, debug, binned)
+                                geomBuffer, imgBuffer, num_rendered, max_tile_len, out_color, debug, binned,
+                                zero_records=zero_records)
     return out_color, binningBuffer
 
 
 def _render(background, colors, radii, geomBuffer, imgBuffer, num_rendered, max_tile_len, out_color, debug, binned=None,
-            stream=None):
+            stream=None, zero_records=True):
     """gh_forward_render into `out_color` on prepared tensors, inside their device's context -> binningBuffer.
     `binned`: the buffer the first phase emitted into (then used as it is), or None: a buffer of the exact size is
-    allocated and emit runs here.  `stream`: the device's current stream (_capi._stream), if the caller has it."""
+    allocated and emit runs here.  `stream`: the device's current stream (_capi._stream), if the caller has it.
+    `zero_records`: the blend clears the accumulation records (see _forward_flags)."""
     lib = _capi.load()
     device = colors.device
     H, W = int(out_color.size(1)), int(out_color.size(2))
@@ -204,9 +209,28 @@ def _render(background, colors, radii, geomBuffer, imgBuffer, num_rendered, max_
     _capi.check(lib.gh_forward_render(
         int(colors.shape[0]), W, H, _ptr(background), _ptr(colors), _ptr(radii),
         _ptr(geomBuffer), _ptr(binningBuffer), _ptr(imgBuffer),
-        int(num_rendered), int(max_tile_len), int(binned is not None), _ptr(out_color), int(bool(debug)),
-        stream if stream is not None else _stream(device)))
+        int(num_rendered), int(max_tile_len), int(binned is not None), _ptr(out_color),
+        _forward_flags(geomBuffer, zero_records, debug), stream if stream is not None else _stream(device)))
     return binningBuffer
+
+
+# The fast blend backward sums into the accumulation records of the geometry workspace, so they must be zero when it
+# starts.  A forward that clears them (GH_FLAG_ZERO_RECORDS) marks the workspace tensor; the first backward on it takes
+# the mark and skips its own clearing pass (GH_FLAG_RECORDS_ZEROED).  A second backward on the same forward
+# (retain_graph=True), or one on a workspace whose forward did not clear the records, finds no mark and clears them.
+# A forward without the flag leaves the records, and so the mark, as they were.
+def _forward_flags(geomBuffer: torch.Tensor, zero_records: bool, debug: bool = False) -> int:
+    """The flags word of a forward render on `geomBuffer`; marks it when the records are cleared."""
+    if zero_records:
+        geomBuffer._gh_records_zeroed = True
+    return (_capi.GH_FLAG_ZERO_RECORDS if zero_records else 0) | (_capi.GH_FLAG_DEBUG if debug else 0)
+
+
+def _backward_flags(geomBuffer: torch.Tensor, debug: bool = False) -> int:
+    """The flags word of a backward on `geomBuffer`; takes the forward's mark (the records are consumed)."""
+    zeroed = bool(getattr(geomBuffer, "_gh_records_zeroed", False))
+    geomBuffer._gh_records_zeroed = False
+    return (_capi.GH_FLAG_RECORDS_ZEROED if zeroed else 0) | (_capi.GH_FLAG_DEBUG if debug else 0)
 
 
 # ------------------------------------------------------------------------------------------------ capturable forward
@@ -220,9 +244,9 @@ def binning_workspace(capacity: int, device: torch.device) -> torch.Tensor:
 
 
 def forward_render_capturable(background, colors, geomBuffer, binningBuffer, imgBuffer, capacity: int,
-                              image_height: int, image_width: int) -> torch.Tensor:
+                              image_height: int, image_width: int, zero_records: bool = True) -> torch.Tensor:
     """gh_forward_render_capturable on the workspaces of projection.project_forward_binned_capturable -> out_color
-    (C,H,W)."""
+    (C,H,W).  `zero_records` as in rasterize_gaussians."""
     device = colors.device
     with torch.cuda.device(device):
         out_color = torch.empty((NUM_CHANNELS, int(image_height), int(image_width)), dtype=torch.float32, device=device)
@@ -230,7 +254,7 @@ def forward_render_capturable(background, colors, geomBuffer, binningBuffer, img
         _capi.check(_capi.load().gh_forward_render_capturable(
             int(colors.shape[0]), int(image_width), int(image_height), int(capacity),
             _ptr(_prep(background, "background", device)), _ptr(colors), _ptr(geomBuffer), _ptr(binningBuffer),
-            _ptr(imgBuffer), _ptr(out_color), 0, _stream(device)))
+            _ptr(imgBuffer), _ptr(out_color), _forward_flags(geomBuffer, zero_records), _stream(device)))
     return out_color
 
 
@@ -251,8 +275,8 @@ def backward_records_capturable(background, colors, radii, geomBuffer, binningBu
         _capi.check(lib.gh_backward_capturable(
             P, W, H, int(capacity), _ptr(_prep(background, "background", device)),
             _ptr(_prep(colors, "colors", device, align=8)), _ptr(radii), _ptr(geomBuffer), _ptr(binningBuffer),
-            _ptr(imgBuffer), _ptr(_prep(dL_dout_color, "dL_dout_color", device)), 0, _stream(device),
-            _ptr(det_buffer), det_bytes))
+            _ptr(imgBuffer), _ptr(_prep(dL_dout_color, "dL_dout_color", device)), _backward_flags(geomBuffer),
+            _stream(device), _ptr(det_buffer), det_bytes))
 
 
 def alloc_grad_arena(P: int, device: torch.device, zero: bool = True, storage: torch.Tensor | None = None):
@@ -304,7 +328,7 @@ def _backward(background, means3D, radii, colors, scales, rotations, scale_modif
             _ptr(dL_dout_color),
             _ptr(g.get("means2D")), _ptr(g.get("conic")), _ptr(g.get("opacity")), _ptr(g.get("colors")),
             _ptr(g.get("means3D")), _ptr(g.get("cov3D")), _ptr(dL_dsh), _ptr(g.get("scales")), _ptr(g.get("rotations")),
-            int(bool(debug)), _stream(device), _ptr(det_buffer), det_bytes))
+            _backward_flags(geomBuffer, debug), _stream(device), _ptr(det_buffer), det_bytes))
 
 
 def rasterize_gaussians_backward_arena(

@@ -22,6 +22,11 @@ GH_E_NO_COLORS = 2
 GH_E_CUDA = 3
 GH_E_PREFILTERED = 4
 
+# bits of the `flags` word of gh_forward_render, gh_backward and their capturable variants (gh_rasterizer.h)
+GH_FLAG_DEBUG = 1
+GH_FLAG_ZERO_RECORDS = 2
+GH_FLAG_RECORDS_ZEROED = 4
+
 ABI_VERSION = 6
 
 _p = C.c_void_p
@@ -67,7 +72,7 @@ SIGNATURES = {
         C.POINTER(_i), C.POINTER(_i), C.POINTER(_i),   # num_rendered max_tile_len emitted
         _i, _p]),                            # debug stream
     "gh_forward_render": (_i, [
-        _i, _i, _i, _p, _p, _p, _p, _p, _p, _i, _i, _i, _p, _i, _p]),     # ... num_rendered max_tile_len emitted ...
+        _i, _i, _i, _p, _p, _p, _p, _p, _p, _i, _i, _i, _p, _i, _p]),     # ... num_rendered max_tile_len emitted out flags stream
     "gh_backward": (_i, [
         _i, _i, _i, _i, _i, _i,              # P D M R width height
         _p,                                  # background
@@ -81,7 +86,7 @@ SIGNATURES = {
         _p,                                  # dL_dpix
         _p, _p, _p, _p,                      # dL_dmean2D dL_dconic dL_dopacity dL_dcolor
         _p, _p, _p, _p, _p,                  # dL_dmean3D dL_dcov3D dL_dsh dL_dscale dL_drot
-        _i, _p,                              # debug stream
+        _i, _p,                              # flags stream
         _p, _sz]),                           # det_buffer det_bytes (NULL, 0: the fast path)
     "gh_mark_visible": (_i, [_i, _p, _p, _p, _p, _p]),
     "gh_adam_step": (_i, [_i, _p, _p, _p, _p, _p, _p, _d, _d, _f, _i, _p, _p, _p, _p]),

@@ -97,7 +97,11 @@ __global__ void gh_export_geom_kernel(int P, const GhGeo* __restrict__ geo, floa
 // The read-back of R: one thread copies ctrl into the caller's pinned host slot (mapped into the device's address space
 // under unified addressing).  A kernel rather than cudaMemcpyAsync: the copy engine's hand-offs from the tile scan and
 // back to emit cost more than the copy itself.
-__global__ void gh_ctrl_readback_kernel(const GhCtrl* __restrict__ ctrl, GhCtrl* host) { *host = *ctrl; }
+__global__ void gh_ctrl_readback_kernel(const GhCtrl* __restrict__ ctrl, GhCtrl* host) {
+    gh_pdl_wait();                                    // ctrl is the tile scan's
+    gh_pdl_trigger();
+    *host = *ctrl;
+}
 
 }  // namespace
 
@@ -158,7 +162,7 @@ int gh_forward_phase1(const char* who, int P, int width, int height, char* geom_
     cudaEvent_t ready = nullptr;
     rc = gh_cuda_status(who, "create the read-back event", cudaEventCreateWithFlags(&ready, cudaEventDisableTiming));
     if (rc == GH_OK) {
-        gh_ctrl_readback_kernel<<<1, 1, 0, stream>>>(img.ctrl, h);
+        gh_launch_pdl(gh_ctrl_readback_kernel, 1, 1, 0, stream, img.ctrl, h);
         rc = gh_launch_status(who, 1);
     }
     if (rc == GH_OK) rc = gh_cuda_status(who, "record the read-back event", cudaEventRecord(ready, stream));
@@ -302,9 +306,10 @@ int gh_forward_render(
     int P, int width, int height,
     const float* background, const float* colors_precomp, const int* radii,
     char* geom_buffer, char* binning_buffer, char* img_buffer,
-    int num_rendered, int max_tile_len, int emitted, float* out_color, int debug, gh_stream_t stream_)
+    int num_rendered, int max_tile_len, int emitted, float* out_color, int flags, gh_stream_t stream_)
 {
     cudaStream_t stream = (cudaStream_t)stream_;
+    const int debug = flags & GH_FLAG_DEBUG;
     gh_clear_error();
     if (P <= 0 || width <= 0 || height <= 0 || num_rendered < 0) return gh_set_error(GH_E_INVALID_ARG, "gh_forward_render: bad sizes");
     if (!background || !colors_precomp || !radii || !geom_buffer || !img_buffer || !out_color || (num_rendered > 0 && !binning_buffer))
@@ -329,7 +334,8 @@ int gh_forward_render(
     }
     {
         GhStageTimer t(GH_ST_BLEND_FWD, stream);
-        gh_launch_blend_forward(width, height, gx, gy, geom, img, bin, colors_precomp, background, out_color, stream);
+        gh_launch_blend_forward(width, height, gx, gy, geom, img, bin, colors_precomp, background, out_color,
+                                P, (flags & GH_FLAG_ZERO_RECORDS) != 0, stream);
         g_launches += 1;
     }
     GH_STAGE("gh_forward_render", stream, debug, "blend forward");
@@ -348,10 +354,11 @@ int gh_backward(
     const float* dL_dpix,
     float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor,
     float* dL_dmean3D, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot,
-    int debug, gh_stream_t stream_, char* det_buffer, size_t det_bytes)
+    int flags, gh_stream_t stream_, char* det_buffer, size_t det_bytes)
 {
     (void)D; (void)M; (void)shs; (void)campos; (void)dL_dsh;
     cudaStream_t stream = (cudaStream_t)stream_;
+    const int debug = flags & GH_FLAG_DEBUG;
     gh_clear_error();
     if (P <= 0 || width <= 0 || height <= 0 || R < 0) return gh_set_error(GH_E_INVALID_ARG, "gh_backward: bad sizes");
     if (det_buffer == nullptr && det_bytes != 0)
@@ -418,8 +425,10 @@ int gh_backward(
         }
     } else if (R > 0) {
         GhStageTimer t(GH_ST_BLEND_BWD, stream);
-        cudaError_t e = cudaMemsetAsync(geom.acc16, 0, (size_t)P * 64, stream);
-        if (e != cudaSuccess) return gh_cuda_status("gh_backward", "memset(accumulation records)", e);
+        if (!(flags & GH_FLAG_RECORDS_ZEROED)) {       // otherwise the forward's blend cleared them
+            cudaError_t e = cudaMemsetAsync(geom.acc16, 0, (size_t)P * 64, stream);
+            if (e != cudaSuccess) return gh_cuda_status("gh_backward", "memset(accumulation records)", e);
+        }
         gh_launch_blend_backward(width, height, gx, gy, geom, img, bin, colors_precomp, background, dL_dpix, stream);
         g_launches += 1;
         if (conic_precomp != nullptr && !keep_records) {   // otherwise the geometry backward unpacks the records itself
@@ -445,12 +454,12 @@ int gh_forward_render_capturable(
     int P, int width, int height, long long capacity,
     const float* background, const float* colors_precomp,
     char* geom_buffer, char* binning_buffer, char* img_buffer,
-    float* out_color, int debug, gh_stream_t stream_)
+    float* out_color, int flags, gh_stream_t stream_)
 {
     const char* who = "gh_forward_render_capturable";
     cudaStream_t stream = (cudaStream_t)stream_;
     gh_clear_error();
-    int rc = gh_check_capturable(who, debug);
+    int rc = gh_check_capturable(who, flags & GH_FLAG_DEBUG);
     if (rc == GH_OK) rc = gh_check_capacity(who, capacity);
     if (rc != GH_OK) return rc;
     if (P <= 0 || width <= 0 || height <= 0) return gh_set_error(GH_E_INVALID_ARG, "%s: bad sizes", who);
@@ -461,7 +470,8 @@ int gh_forward_render_capturable(
     GhImgWS img = GhImgWS::carve(img_buffer, (size_t)width * height, (size_t)T);
     GhBinWS bin = GhBinWS::carve(binning_buffer, (size_t)capacity);
     const int n = gh_launch_tile_sort_capturable(T, (unsigned int)capacity, img, bin, stream);
-    gh_launch_blend_forward(width, height, gx, gy, geom, img, bin, colors_precomp, background, out_color, stream);
+    gh_launch_blend_forward(width, height, gx, gy, geom, img, bin, colors_precomp, background, out_color,
+                            P, (flags & GH_FLAG_ZERO_RECORDS) != 0, stream);
     return gh_launch_status(who, n + 1);
 }
 
@@ -469,12 +479,12 @@ int gh_backward_capturable(
     int P, int width, int height, long long capacity,
     const float* background, const float* colors_precomp, const int* radii,
     char* geom_buffer, char* binning_buffer, char* img_buffer,
-    const float* dL_dpix, int debug, gh_stream_t stream_, char* det_buffer, size_t det_bytes)
+    const float* dL_dpix, int flags, gh_stream_t stream_, char* det_buffer, size_t det_bytes)
 {
     const char* who = "gh_backward_capturable";
     cudaStream_t stream = (cudaStream_t)stream_;
     gh_clear_error();
-    int rc = gh_check_capturable(who, debug);
+    int rc = gh_check_capturable(who, flags & GH_FLAG_DEBUG);
     if (rc == GH_OK) rc = gh_check_capacity(who, capacity);
     if (rc != GH_OK) return rc;
     if (P <= 0 || width <= 0 || height <= 0) return gh_set_error(GH_E_INVALID_ARG, "%s: bad sizes", who);
@@ -499,8 +509,10 @@ int gh_backward_capturable(
         gh_launch_det_gather(P, geom, det, stream);
         return gh_launch_status(who, n + 2);
     }
-    rc = gh_cuda_status(who, "memset(accumulation records)", cudaMemsetAsync(geom.acc16, 0, (size_t)P * 64, stream));
-    if (rc != GH_OK) return rc;
+    if (!(flags & GH_FLAG_RECORDS_ZEROED)) {
+        rc = gh_cuda_status(who, "memset(accumulation records)", cudaMemsetAsync(geom.acc16, 0, (size_t)P * 64, stream));
+        if (rc != GH_OK) return rc;
+    }
     gh_launch_blend_backward(width, height, gx, gy, geom, img, bin, colors_precomp, background, dL_dpix, stream);
     return gh_launch_status(who, 1);
 }

@@ -59,6 +59,8 @@ gh_tile_scan_kernel(int T, const uint32_t* __restrict__ tile_count, uint32_t* __
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     const unsigned rank = cluster.block_rank();
     if (tid < 128) s_hist[tid] = 0u;
+    gh_pdl_wait();                              // tile_count is the preprocess kernel's histogram
+    gh_pdl_trigger();
     uint32_t tmax = 0, carry = 0;
     __syncthreads();
     int round = 0;
@@ -201,6 +203,8 @@ gh_emit_kernel(int P, const int* __restrict__ radii, const GhGeo* __restrict__ g
                const float* __restrict__ depth, uint32_t* __restrict__ tile_cursor,
                uint64_t* __restrict__ inst, int gx, int gy, const GhCtrl* __restrict__ ctrl, uint32_t capacity)
 {
+    gh_pdl_wait();                                 // every input comes from the preprocess kernel and the scan
+    gh_pdl_trigger();
     if (ctrl->num_rendered > capacity) return;     // uniform over the grid
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;
     const int lane = threadIdx.x & 31;
@@ -367,14 +371,15 @@ gh_capacity_guard_kernel(int P, int* __restrict__ radii, int T, uint2* __restric
 
 void gh_launch_tile_scan(int T, GhImgWS img, cudaStream_t stream)
 {
-    gh_tile_scan_kernel<<<GH_SCAN_CTAS, GH_SCAN_THREADS, 0, stream>>>(T, img.tile_count, img.tile_cursor, img.ranges, img.tile_perm, img.ctrl);
+    gh_launch_pdl(gh_tile_scan_kernel, GH_SCAN_CTAS, GH_SCAN_THREADS, 0, stream,
+                  T, img.tile_count, img.tile_cursor, img.ranges, img.tile_perm, img.ctrl);
 }
 
 void gh_launch_emit(int P, const int* radii, GhGeomWS geom, GhImgWS img, GhBinWS bin, unsigned int capacity,
                     int gx, int gy, cudaStream_t stream)
 {
-    gh_emit_kernel<<<(P + 255) / 256, 256, 0, stream>>>(P, radii, geom.geo, geom.depth,
-                                                        img.tile_cursor, bin.inst, gx, gy, img.ctrl, capacity);
+    gh_launch_pdl(gh_emit_kernel, (P + 255) / 256, 256, 0, stream,
+                  P, radii, geom.geo, geom.depth, img.tile_cursor, bin.inst, gx, gy, img.ctrl, capacity);
 }
 
 int gh_launch_tile_sort(int T, unsigned int max_tile_len, long long R, GhImgWS img, GhBinWS bin, cudaStream_t stream)

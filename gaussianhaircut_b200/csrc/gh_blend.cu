@@ -33,6 +33,8 @@
 #include "gh_common.cuh"
 #include "gh_kernels.h"
 
+#include <atomic>
+
 #define GH_HALF_C (GH_NUM_CHANNELS / 2)
 
 // ---- build-time tunables (defaults = the measured best; tools/bench_variants.py rebuilds with -D overrides)
@@ -235,7 +237,8 @@ gh_blend_forward_kernel(const uint2* __restrict__ ranges, const uint32_t* __rest
                         const GhGeo* __restrict__ geo, const float* __restrict__ features,
                         int W, int H, int gx, const float* __restrict__ bg,
                         float* __restrict__ final_T, uint32_t* __restrict__ n_contrib,
-                        float* __restrict__ out)
+                        float* __restrict__ out,
+                        float4* __restrict__ zero_records, size_t zero_n)   // NULL, or the P * 4 float4 of acc16
 {
     // Forward needs no cross-pixel communication, so every lane walks the list of ITS OWN pixel pair (the union of
     // the two pixels' lists): a lane only ever touches Gaussians whose alpha >= 1/255 footprint (conservatively)
@@ -243,6 +246,9 @@ gh_blend_forward_kernel(const uint2* __restrict__ ranges, const uint32_t* __rest
     extern __shared__ __align__(16) unsigned char gh_fwd_smem[];
     GhStage<GH_FWD_CHUNK>& st = *reinterpret_cast<GhStage<GH_FWD_CHUNK>*>(gh_fwd_smem);
     uint32_t* pairbits = reinterpret_cast<uint32_t*>(gh_fwd_smem + sizeof(st));   // [word][pair] (GH_FWD_WORDS x 128)
+
+    gh_pdl_wait();                                    // the lists, ranges and tile order come from emit and the scan
+    gh_pdl_trigger();
 
     const int tile = (int)tile_perm[blockIdx.x];      // heaviest tiles first
     const int tx = tile % gx, ty = tile / gx;
@@ -419,6 +425,20 @@ gh_blend_forward_kernel(const uint2* __restrict__ ranges, const uint32_t* __rest
 #pragma unroll
         for (int ch = 0; ch < GH_NUM_CHANNELS; ch++)
             out[ch * plane + pix] = GH_FMA(Tr, __ldg(bg + ch), r ? C[ch].y : C[ch].x);
+    }
+
+    // Clear the backward's accumulation records, so that the blend backward needs no clearing pass of its own.  The
+    // first quarter of the CTAs -- the heaviest tiles, launched first -- take one contiguous slice each: their
+    // traversal is bound by latency and leaves the memory pipe idle, whereas the light and empty tiles that run last
+    // are bound by their image stores (zeroing in every CTA cost ~9 us of blend forward on the bench step, in the
+    // prologue or at the end alike).  At the end, after the CTA's own stores: CTAs finish at different times, so the
+    // clearing spreads over the kernel.
+    const unsigned nzero = max(1u, gridDim.x / 4);
+    if (zero_records != nullptr && blockIdx.x < nzero) {
+        const size_t per = (zero_n + nzero - 1) / nzero;
+        const size_t end = min(zero_n, per * (blockIdx.x + 1));
+        const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
+        for (size_t i = per * blockIdx.x + tid; i < end; i += GH_FWD_THREADS) zero_records[i] = z;
     }
 }
 
@@ -642,6 +662,8 @@ gh_blend_backward_kernel(const uint2* __restrict__ ranges, const uint32_t* __res
     __shared__ uint32_t s_glast[kBwdBlocks];              // per block: deepest list position any of its pixels blended
     __shared__ uint8_t s_perm[GH_BWD_THREADS / 32][kBwdBlocks];   // per warp (redundant copies): rank -> block
 
+    gh_pdl_wait();                                    // every input but the caller's comes from the forward
+    gh_pdl_trigger();
     const int tile = (int)tile_perm[blockIdx.x];      // heaviest tiles first
     const int tx = tile % gx, ty = tile / gx;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -910,6 +932,8 @@ gh_unpack_grads_kernel(int P, const float* __restrict__ acc16, float* __restrict
 {
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= P) return;
+    gh_pdl_wait();                                    // acc16 comes from the blend backward
+    gh_pdl_trigger();
     const float4* a = reinterpret_cast<const float4*>(acc16 + (size_t)idx * 16);
     const float4 a0 = a[0], a1 = a[1], a2 = a[2], a3 = a[3];
     float2* dc = reinterpret_cast<float2*>(dL_dcolor + (size_t)idx * GH_NUM_CHANNELS);
@@ -1025,19 +1049,35 @@ gh_det_gather_kernel(int P, const uint32_t* __restrict__ off, const float4* __re
     acc16[4 * i + q] = a;
 }
 
+// The shared-memory attributes of a blend kernel, set once per device (bit `dev` of `devices`; devices past 63 set them
+// on every launch): the forward's launch sits on the host's path from the read-back of R to the GPU's next work, where
+// each runtime call is time the GPU may spend waiting.
+template <typename Kernel>
+void gh_blend_smem_once(Kernel kernel, int smem, std::atomic<unsigned long long>& devices)
+{
+    int dev = 0;
+    cudaGetDevice(&dev);
+    const unsigned long long bit = dev < 64 ? 1ull << dev : 0ull;
+    if (devices.load(std::memory_order_relaxed) & bit) return;
+    if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) == cudaSuccess &&
+        cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100) == cudaSuccess)
+        devices.fetch_or(bit);
+}
+std::atomic<unsigned long long> g_fwd_smem_set{0}, g_bwd_smem_set{0}, g_bwd_det_smem_set{0};
+
 }  // namespace
 
 void gh_launch_blend_forward(int W, int H, int gx, int gy, GhGeomWS geom, GhImgWS img, GhBinWS bin,
                              const float* features, const float* bg, float* out_color,
-                             cudaStream_t stream)
+                             int P, bool zero_records, cudaStream_t stream)
 {
     // 6 CTAs of 128 threads per SM: 34 KB of dynamic shared memory each (the in-CTA sort's buffers, the largest use)
     // out of the largest carve-out
     const int smem = (int)kFwdSmemBytes;
-    cudaFuncSetAttribute(gh_blend_forward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    cudaFuncSetAttribute(gh_blend_forward_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
-    gh_blend_forward_kernel<<<gx * gy, GH_FWD_THREADS, smem, stream>>>(img.ranges, img.tile_perm, bin.inst, geom.geo, features,
-                                                         W, H, gx, bg, img.final_T, img.n_contrib, out_color);
+    gh_blend_smem_once(gh_blend_forward_kernel, smem, g_fwd_smem_set);
+    gh_launch_pdl(gh_blend_forward_kernel, gx * gy, GH_FWD_THREADS, smem, stream,
+                  img.ranges, img.tile_perm, bin.inst, geom.geo, features, W, H, gx, bg, img.final_T, img.n_contrib,
+                  out_color, zero_records ? reinterpret_cast<float4*>(geom.acc16) : nullptr, (size_t)P * 4);
 }
 
 void gh_launch_blend_backward(int W, int H, int gx, int gy, GhGeomWS geom, GhImgWS img, GhBinWS bin,
@@ -1045,11 +1085,10 @@ void gh_launch_blend_backward(int W, int H, int gx, int gy, GhGeomWS geom, GhImg
                               cudaStream_t stream)
 {
     const int smem = (int)sizeof(GhStageB);
-    cudaFuncSetAttribute(gh_blend_backward_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    cudaFuncSetAttribute(gh_blend_backward_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
-    gh_blend_backward_kernel<false><<<gx * gy, GH_BWD_THREADS, smem, stream>>>(img.ranges, img.tile_perm, bin.inst, geom.geo, features,
-                                                          W, H, gx, bg, img.final_T, img.n_contrib, dL_dpix,
-                                                          geom.acc16, GhDetArgs{});
+    gh_blend_smem_once(gh_blend_backward_kernel<false>, smem, g_bwd_smem_set);
+    gh_launch_pdl(gh_blend_backward_kernel<false>, gx * gy, GH_BWD_THREADS, smem, stream,
+                  img.ranges, img.tile_perm, bin.inst, geom.geo, features, W, H, gx, bg, img.final_T, img.n_contrib,
+                  dL_dpix, geom.acc16, GhDetArgs{});
 }
 
 int gh_launch_det_offsets(int P, int gx, int gy, const int* radii, GhGeomWS geom, GhDetWS det, cudaStream_t stream)
@@ -1066,8 +1105,7 @@ void gh_launch_blend_backward_det(int W, int H, int gx, int gy, const int* radii
                                   cudaStream_t stream)
 {
     const int smem = (int)(sizeof(GhStageB) + kBwdDetPartBytes);
-    cudaFuncSetAttribute(gh_blend_backward_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    cudaFuncSetAttribute(gh_blend_backward_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    gh_blend_smem_once(gh_blend_backward_kernel<true>, smem, g_bwd_det_smem_set);
     const GhDetArgs d{radii, det.off, reinterpret_cast<float4*>(det.rows), gy};
     gh_blend_backward_kernel<true><<<gx * gy, GH_BWD_THREADS, smem, stream>>>(img.ranges, img.tile_perm, bin.inst, geom.geo, features,
                                                          W, H, gx, bg, img.final_T, img.n_contrib, dL_dpix,
@@ -1085,7 +1123,6 @@ void gh_launch_unpack_grads(int P, GhGeomWS geom, float* dL_dmean2D, float* dL_d
                             float* dL_dcolor, float* dL_dmean3D, float* dL_dcov3D, float* dL_dscale, float* dL_drot,
                             cudaStream_t stream)
 {
-    gh_unpack_grads_kernel<<<(P + 255) / 256, 256, 0, stream>>>(P, geom.acc16, dL_dmean2D, dL_dconic,
-                                                                dL_dopacity, dL_dcolor, dL_dmean3D, dL_dcov3D,
-                                                                dL_dscale, dL_drot);
+    gh_launch_pdl(gh_unpack_grads_kernel, (P + 255) / 256, 256, 0, stream,
+                  P, geom.acc16, dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolor, dL_dmean3D, dL_dcov3D, dL_dscale, dL_drot);
 }

@@ -223,6 +223,31 @@ __device__ __forceinline__ GhGeo gh_geo_not_rendered() {
     return g;
 }
 
+// ---- programmatic dependent launch along the step's kernel chain ---------------------------------------------------
+// gh_launch_pdl lets the kernel's CTAs start while the previous kernel in the stream is still finishing its last wave,
+// so that launch, CTA rasterization and the kernel's own prologue overlap the predecessor's tail.  The contract every
+// kernel launched this way keeps:
+//   * before gh_pdl_wait() it reads nothing an earlier kernel of the stream may still be writing, and writes nothing;
+//   * gh_pdl_wait() returns when every earlier kernel has completed and its writes are visible;
+//   * gh_pdl_trigger() comes after gh_pdl_wait() -- so a dependent that starts early only ever overlaps kernels whose
+//     own predecessors have completed -- and only allows the next kernel to be scheduled: it makes none of this
+//     kernel's writes visible; the next kernel's gh_pdl_wait() does.
+// Without the launch attribute (a plain <<<>>> launch, or an event between the two kernels) both are no-ops.  Stream
+// capture records the launch as a programmatic graph edge.
+template <typename... KArgs, typename... Args>
+static inline void gh_launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
+                                 Args... args) {
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = stream;
+    cfg.attrs = attr; cfg.numAttrs = 1;
+    cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);   // errors surface through cudaGetLastError
+}
+__device__ __forceinline__ void gh_pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+__device__ __forceinline__ void gh_pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+
 // ---- row spans staged through shared memory (gh_preprocess_backward_kernel) ------------------------------------------
 // The rows [row0, row0 + n) of a row-major (P, K) float array are ONE contiguous span of K * n floats.  A CTA moves it
 // between global and shared memory with 16-byte accesses instead of K strided scalar accesses per thread: span element

@@ -32,9 +32,10 @@ void gh_launch_capacity_guard(int P, int* radii, int T, GhImgWS img, unsigned in
                               unsigned int* num_rendered_out, cudaStream_t stream);
 int gh_launch_tile_sort_capturable(int T, unsigned int capacity, GhImgWS img, GhBinWS bin, cudaStream_t stream);
 
+// zero_records: the kernel also clears geom.acc16 (P records) for the fast blend backward
 void gh_launch_blend_forward(int W, int H, int gx, int gy, GhGeomWS geom, GhImgWS img, GhBinWS bin,
                              const float* features, const float* bg, float* out_color,
-                             cudaStream_t stream);
+                             int P, bool zero_records, cudaStream_t stream);
 
 // accumulates into geom.acc16 (must be zero on entry)
 void gh_launch_blend_backward(int W, int H, int gx, int gy, GhGeomWS geom, GhImgWS img, GhBinWS bin,

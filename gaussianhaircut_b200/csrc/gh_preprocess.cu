@@ -29,6 +29,10 @@ gh_preprocess_kernel(int P,
 {
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;
     const bool valid = idx < P;
+    // the inputs may come from the kernel just before (the optimizer, the projection), and the tile histogram from the
+    // memset before this launch: nothing is read before the wait
+    gh_pdl_wait();
+    gh_pdl_trigger();
 
     // radius 0 <=> "not rendered" (forward.cu:190-191)
     int out_radius = 0;
@@ -147,7 +151,7 @@ void gh_launch_preprocess(int P, const float* means3D, const float* scales, floa
 {
     const float focal_y = H / (2.0f * tan_fovy);   // rasterizer_impl.cu:224-225
     const float focal_x = W / (2.0f * tan_fovx);
-    gh_preprocess_kernel<<<(P + 127) / 128, 128, 0, stream>>>(
+    gh_launch_pdl(gh_preprocess_kernel, (P + 127) / 128, 128, 0, stream,
         P, means3D, scales, scale_modifier, rotations, opacities, cov3D_precomp, conic_precomp,
         viewmatrix, projmatrix, W, H, tan_fovx, tan_fovy, focal_x, focal_y, radii,
         geom.geo, geom.depth, img.tile_count, img.ctrl, gx, gy, prefiltered);

@@ -51,12 +51,16 @@ gh_preprocess_backward_kernel(int P, const float* __restrict__ means3D, const in
     const float* g_acc = acc16 + (size_t)row0 * 16;
     const float* g_mean = means3D + (size_t)row0 * 3;
     const float* g_c3 = from_scale_rot ? scales + (size_t)row0 * 3 : cov3D_precomp + (size_t)row0 * 6;
-    gh_span_load_async(s_acc, g_acc, 16 * n);
+    // the caller's inputs are requested before the wait: the blend backward (or the unpack) that runs before this
+    // kernel writes none of them, and the kernels before it have completed
     gh_span_load_async(s_mean, g_mean, 3 * n);
     gh_span_load_async(s_c3, g_c3, (from_scale_rot ? 3 : 6) * n);
     const bool rendered = valid && radii[idx] > 0;
     float4 q = make_float4(0.f, 0.f, 0.f, 0.f);
     if (rendered && from_scale_rot) q = reinterpret_cast<const float4*>(rotations)[idx];
+    gh_pdl_wait();                               // acc16 is the blend backward's output
+    gh_pdl_trigger();
+    gh_span_load_async(s_acc, g_acc, 16 * n);
     gh_span_wait();
     __syncthreads();
     // acc16 rows are 64-byte aligned (GhGeomWS), so this thread's record is four aligned float4 in shared memory
@@ -279,7 +283,7 @@ void gh_launch_preprocess_backward(int P, const float* means3D, const int* radii
     if (conic_precomp != nullptr) return;   // reference: geometry backward is a no-op in this mode (caller unpacks)
     const float focal_y = H / (2.0f * tan_fovy);
     const float focal_x = W / (2.0f * tan_fovx);
-    gh_preprocess_backward_kernel<<<(P + GH_PBWD_THREADS - 1) / GH_PBWD_THREADS, GH_PBWD_THREADS, 0, stream>>>(
+    gh_launch_pdl(gh_preprocess_backward_kernel, (P + GH_PBWD_THREADS - 1) / GH_PBWD_THREADS, GH_PBWD_THREADS, 0, stream,
         P, means3D, radii, scales, scale_modifier, rotations, cov3D_precomp, viewmatrix, projmatrix,
         focal_x, focal_y, tan_fovx, tan_fovy, acc16, dL_dmean2D, dL_dconic, dL_dopacity, dL_dcolor,
         dL_dmean3D, dL_dcov3D, dL_dscale, dL_drot);

@@ -99,11 +99,13 @@ class _FusedRender(torch.autograd.Function):
         pi = projection.pack_inputs(xyz, scaling, rotation, dirs, f_dc, f_rest, opacity, label, conf, viewmatrix, projmatrix,
                                     campos, st["tanx"], st["tany"], st["W"], st["H"], st["sh_degree"], st["mod"], st["cfg"])
         bg = st["bg"]
+        zero = any(ctx.needs_input_grad)    # only a forward with a backward needs cleared accumulation records
         if n_head == 0 and P_own > 0 and not st["debug"]:
             # one pass over the Gaussians does the projection AND the rasterizer's preprocess + tile histogram
             out, radii, geom, img, R, max_len, binned = projection.project_forward_binned(pi, means2D_out=viewspace.detach(),
                                                                                         binning=True)
-            color, binning = _C.forward_render(bg, out["colors"], radii, geom, img, R, max_len, st["H"], st["W"], binned=binned)
+            color, binning = _C.forward_render(bg, out["colors"], radii, geom, img, R, max_len, st["H"], st["W"], binned=binned,
+                                               zero_records=zero)
             ctx.pi, ctx.st, ctx.R, ctx.n_head, ctx.hp = pi, st, R, 0, None
             ctx.bufs = (pi.xyz, out["colors"], out["conic"], out["visible"], radii, geom, binning, img)
             ctx.mark_non_differentiable(radii)
@@ -125,7 +127,7 @@ class _FusedRender(torch.autograd.Function):
         R, color, radii, geom, binning, img = _C.rasterize_gaussians(
             bg, means3D, _EMPTY, out["colors"], out["opacity"], _EMPTY, _EMPTY, st["mod"], _EMPTY, out["conic"],
             pi.V, pi.Pm, st["tanx"], st["tany"], st["H"], st["W"], _EMPTY, st["sh_degree"], pi.campos,
-            False, st["debug"])            # prefiltered=False: culled Gaussians are still in the list (conic = 0)
+            False, st["debug"], zero_records=zero)   # prefiltered=False: culled Gaussians are still in the list (conic = 0)
         ctx.pi, ctx.st, ctx.R, ctx.n_head = pi, st, R, n_head
         ctx.hp = hp if n_head > 0 else None
         ctx.bufs = (means3D, out["colors"], out["conic"], out["visible"], radii, geom, binning, img)

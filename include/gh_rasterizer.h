@@ -124,10 +124,25 @@ int gh_forward_preprocess(
     int debug, gh_stream_t stream);
 
 /*
+ * Bits of the `flags` word of gh_forward_render, gh_backward and their capturable variants.
+ *   GH_FLAG_DEBUG: synchronise and report after every stage (refused by the capturable variants).
+ *   GH_FLAG_ZERO_RECORDS (forward): the blend forward also clears the P accumulation records of the geometry
+ *     workspace, which the fast blend backward sums into.
+ *   GH_FLAG_RECORDS_ZEROED (backward): the records still hold the zeros of a GH_FLAG_ZERO_RECORDS forward -- no
+ *     backward has run on them since -- so the fast path skips its own clearing pass.  Leave it unset for a second
+ *     backward of the same forward.  The deterministic path assigns every record and ignores it.
+ * A flags word of 0 or 1 means what the former `debug` argument meant.
+ */
+#define GH_FLAG_DEBUG 1
+#define GH_FLAG_ZERO_RECORDS 2
+#define GH_FLAG_RECORDS_ZEROED 4
+
+/*
  * Phase 2 of Rasterizer::forward: binning + per-tile sort + front-to-back blend.
  * out_color is (C, H, W) channel-major, fully overwritten (background included).
  * emitted = 1 skips the bucket scatter that the first phase already ran into binning_buffer (gh_forward_preprocess /
  * gh_project_forward_binned reported *emitted = 1 for this buffer); emitted = 0 runs it here.
+ * flags: GH_FLAG_DEBUG, GH_FLAG_ZERO_RECORDS.
  */
 int gh_forward_render(
     int P, int width, int height,
@@ -136,7 +151,7 @@ int gh_forward_render(
     char* geom_buffer, char* binning_buffer, char* img_buffer,
     int num_rendered, int max_tile_len, int emitted,
     float* out_color,
-    int debug, gh_stream_t stream);
+    int flags, gh_stream_t stream);
 
 /*
  * Rasterizer::backward (rasterizer.h:57-87).  Every element of every non-NULL gradient buffer is
@@ -155,6 +170,7 @@ int gh_forward_render(
  * function of the inputs (bit-identical across runs on the same GPU and build).  It needs det_bytes >=
  * gh_backward_det_workspace_size(P, R) bytes of device memory; a smaller buffer, or det_bytes != 0 without a
  * buffer, is rejected with GH_E_INVALID_ARG before anything is launched.
+ * flags: GH_FLAG_DEBUG, GH_FLAG_RECORDS_ZEROED.
  */
 int gh_backward_det_workspace_size(int P, long long R, size_t* bytes);
 
@@ -172,7 +188,7 @@ int gh_backward(
     const float* dL_dpix,
     float* dL_dmean2D, float* dL_dconic, float* dL_dopacity, float* dL_dcolor,
     float* dL_dmean3D, float* dL_dcov3D, float* dL_dsh, float* dL_dscale, float* dL_drot,
-    int debug, gh_stream_t stream,
+    int flags, gh_stream_t stream,
     char* det_buffer, size_t det_bytes);
 
 /* Rasterizer::markVisible: present[i] = (view-space z of point i > 0.2).  `present` is bool[P]. */
@@ -469,8 +485,8 @@ int gh_project_backward(
  * or writes a binning record at or beyond `capacity`, and every output is still written: the image is the background
  * (final_T = 1, n_contrib = 0), the accumulation records and all gradients are zero.  Pass `status` as the skip_flag
  * of gh_adam_step_capturable so that the iteration's update is skipped on the device, and zero it before each
- * iteration.  Each entry point rejects debug != 0, and any call while the stage timer is on, with GH_E_INVALID_ARG
- * before it launches anything.
+ * iteration.  Each entry point rejects debug != 0 (GH_FLAG_DEBUG in a flags word), and any call while the stage timer
+ * is on, with GH_E_INVALID_ARG before it launches anything.
  *
  * gh_project_forward_binned_capturable: gh_project_forward_binned (non-strand flags; no cov3D) with tan fov from the
  *   device, no read-back and no pinned memory; emit is always enqueued into `binning_buffer`.  num_rendered (device
@@ -479,6 +495,7 @@ int gh_project_backward(
  *   taken on the device: the long-list split and segment sort are always launched, on grids bounded by T and
  *   `capacity`, and their CTAs leave at once when no list exceeds the in-kernel sort's 1792 records.  With the same
  *   inputs and R <= capacity the image, final_T, n_contrib and the sorted lists are bit-identical to gh_forward_render.
+ *   `flags` of these two: GH_FLAG_ZERO_RECORDS / GH_FLAG_RECORDS_ZEROED as for gh_forward_render and gh_backward.
  * gh_backward_capturable: the records-mode blend backward of gh_backward (conic supplied, the four 2-D gradient
  *   outputs NULL): the accumulation records are left in the geometry workspace.  det_buffer selects the deterministic
  *   variant as in gh_backward (records bit-identical to it); NULL the fast one.  An empty or overflowed frame yields
@@ -502,12 +519,12 @@ int gh_forward_render_capturable(
     int P, int width, int height, long long capacity,
     const float* background, const float* colors_precomp,
     char* geom_buffer, char* binning_buffer, char* img_buffer,
-    float* out_color, int debug, gh_stream_t stream);
+    float* out_color, int flags, gh_stream_t stream);
 int gh_backward_capturable(
     int P, int width, int height, long long capacity,
     const float* background, const float* colors_precomp, const int* radii,
     char* geom_buffer, char* binning_buffer, char* img_buffer,
-    const float* dL_dpix, int debug, gh_stream_t stream, char* det_buffer, size_t det_bytes);
+    const float* dL_dpix, int flags, gh_stream_t stream, char* det_buffer, size_t det_bytes);
 int gh_project_backward_capturable(
     int P, int width, int height,
     const float* xyz, const float* scaling, const float* rotation, const float* dirs,
